@@ -2,6 +2,7 @@
 """bench.py -- queries/sec of one training step of the hot path (BASELINE.json configs).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference|reference-cuda] [--config a|b|c|d|e]
+                    [--dump-outputs DIR]
 
 A "step" = scorer forward + fused loss/gradient + scorer backward + gradient all-reduce (N>1) + optimizer step over one
 batch of synthetic MSLR-shaped queries per GPU (weak scaling).  Default --config b = BASELINE.json configs[1], the
@@ -21,6 +22,9 @@ Prints ONE JSON line on rank 0:
   reference_cuda  the same restatement as PyTorch eager on cuda:0 (the reference's `-cuda 0` path), N=1 only
   strong_scaling  (N>1) the same global batch as N=1 split over the ranks
 --impl reference times the CPU restatement alone (rank 0 only); --impl reference-cuda the eager-GPU one.
+--dump-outputs DIR writes what the last timed step computed -- its loss and the parameters the optimizer step left --
+as DIR/<name>.npy (rank 0), so two builds run with the same arguments (hence the same seeded inputs) can be compared
+output for output.
 """
 from __future__ import annotations
 
@@ -161,8 +165,27 @@ def measured_peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"],
                     bf16_tflops_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
-                    sm_max_mhz=d.get("sm_max_mhz", 1965.0), source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, sm_max_mhz=1965.0, source="fallback")
+                    sm_max_mhz=d.get("sm_max_mhz", 1980.0), source="measured")
+    # NVIDIA's H100 SXM data sheet (700 W card; dense BF16): upper bounds, not reached rates
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, sm_max_mhz=1980.0, source="H100 SXM data sheet")
+
+
+DUMP_LIMIT = 64 << 20          # bytes written by --dump-outputs in all
+
+
+def dump_outputs(out_dir, arrays):
+    """Write (name, tensor) pairs as out_dir/<name>.npy in float32 / float64.  An array larger than its share of
+    DUMP_LIMIT is replaced by a fixed, seeded sample of its (flattened) elements."""
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_LIMIT // max(1, len(arrays))
+    for name, t in arrays:
+        a = t.detach().cpu().numpy() if torch.is_tensor(t) else np.asarray(t)
+        if a.dtype not in (np.float32, np.float64):
+            a = a.astype(np.float64)
+        if a.nbytes > share:
+            idx = np.sort(np.random.default_rng(SEED).choice(a.size, share // a.itemsize, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a))
 
 
 # --------------------------------------------------------------------------- #
@@ -195,6 +218,16 @@ def reference_run(cfg, steps, warmup, B, budget_s, device="cpu"):
     return dict(qps=done * B / dt, ms_per_step=1e3 * dt / done, steps=done, B=B, cores=torch.get_num_threads())
 
 
+def power_limit(gpu_index):
+    """The card's enforced power limit in W (part of every absolute number this benchmark reports), or None."""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(gpu_index)],
+                             capture_output=True, text=True, timeout=20).stdout.strip()
+        return float(out)
+    except Exception:
+        return None
+
+
 def host_threads():
     """Threads for the CPU arm: every PHYSICAL core this process may run on (torchrun exports OMP_NUM_THREADS=1, and
     oversubscribing the SMT siblings makes ATen's elementwise kernels several times slower)."""
@@ -225,7 +258,7 @@ def run_reference(args, cfg, device="cpu"):
         "dtype": "f32", "data": "synthetic",
         "config": {"workload": cfg["workload"], "queries_per_step": B, "n_docs": cfg["n"], "n_features": cfg["F"],
                    "device": device,
-                   "sample": "each step is a bounded sample of the workload: one batch of %d queries (the B200 arm steps %d per GPU)" % (B, cfg["B"]),
+                   "sample": "each step is a bounded sample of the workload: one batch of %d queries (the GPU arm steps %d per GPU)" % (B, cfg["B"]),
                    "math": "fp32 ATen kernels"},
         "cpu_baseline": {"value": r["qps"], "unit": "queries/s", "cores": r["cores"], "kind": "port", "sample": sample},
         "e2e": {"value": r["qps"], "unit": "queries/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
@@ -235,7 +268,7 @@ def run_reference(args, cfg, device="cpu"):
 
 
 # --------------------------------------------------------------------------- #
-# B200 arm
+# GPU arm: the ptranking_b200 CUDA implementation
 # --------------------------------------------------------------------------- #
 class HostBatches:
     """Iterable of (ids, X, y) pinned-host batches -- what ranker.train() consumes (the reference's DataLoader contract:
@@ -333,6 +366,9 @@ def run_b200(args, cfg):
     launches = _lib.launch_count() - l0
     value = world * B * args.steps / (ms / 1e3)
     last_loss = float(loss)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, [("loss", loss.double().reshape(1))] +
+                     [("param_%03d" % i, p) for i, p in enumerate(ranker.get_parameters())])
 
     # ---- strong scaling: the N=1 global batch split over the ranks ----------------
     strong = None
@@ -376,7 +412,7 @@ def run_b200(args, cfg):
     cpu = ref_b1 = ref_cuda = None
     if rank == 0 and world == 1 and not args.no_cpu_baseline:
         # GPU-side comparators first: both are (partly) launch-bound, and the worker threads of the CPU runs below keep
-        # spinning for a while after a parallel region -- measured 0.62 ms vs 2.0 ms per B = 1 step depending on the order
+        # spinning for a while after a parallel region, which would slow the launch-bound B = 1 GPU steps
         B1 = max(1, 100 // n)       # the reference's own batching: B = max(1, 100 // n) queries per step (data_utils.py:683-718)
         one = [(X[:B1].contiguous(), y[:B1].contiguous()) for X, y in devb]
         ms1, _ = timed(one, 50, 5)
@@ -391,10 +427,12 @@ def run_b200(args, cfg):
         cpu = {"value": r["qps"], "unit": "queries/s", "cores": r["cores"], "kind": "port",
                "sample": f"{r['steps']} steps x {r['B']} queries x {n} docs (oracle/ref_port.py train_op, fp32 CPU PyTorch ops)"}
         r1 = reference_run(cfg, steps=200, warmup=3, B=B1, budget_s=5.0)
-        ref_b1 = {"queries_per_step": B1, "cpu_port_qps": r1["qps"], "b200_qps": B1 * 50 / (ms1 / 1e3),
-                  "b200_ms_per_step": ms1 / 50, "note": "launch-latency bound on the GPU: ~50 kernel launches per step"}
+        ref_b1 = {"queries_per_step": B1, "cpu_port_qps": r1["qps"], "gpu_qps": B1 * 50 / (ms1 / 1e3),
+                  "gpu_ms_per_step": ms1 / 50, "note": "launch-latency bound on the GPU: ~50 kernel launches per step"}
 
     if rank == 0:
+        props = torch.cuda.get_device_properties(local)
+        l2_bytes = props.L2_cache_size
         line = {
             "metric": cfg["metric"], "value": value, "unit": "queries/s",
             "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms / args.steps,
@@ -405,10 +443,11 @@ def run_b200(args, cfg):
                        "gradient_exchange": ("none (one GPU)" if world == 1 else
                                              "summed inside the optimizer kernel over NVLink peer memory (CUDA IPC), one launch" if getattr(ranker.grad_bucket, "peer", None) is not None
                                              else "ncclAllReduce(SUM) of the flat gradient buffer, then the optimizer kernel"),
-                       "l2": f"inputs (2 x {h2d / 1e6:.0f} MB rotating batches) " + ("larger than" if 2 * h2d > 126e6 else "NOT larger than") + " the 126 MB L2",
+                       "l2": f"inputs (2 x {h2d / 1e6:.0f} MB rotating batches) " + ("larger than" if 2 * h2d > l2_bytes else "NOT larger than") + f" the {l2_bytes / 1e6:.0f} MB L2",
                        "normalisation": "BN (reference default, batch statistics" + (", synchronised over ranks)" if b200dist.sync_bn_active() else " per rank)") if cfg["sf"]["sf_id"] == "pointsf" else "none (listsf default)",
                        "math": ("GEMM operands rounded to bf16, fp32 accumulate" if cfg["math"] == "bf16" else
-                                "fp32 in/out; Linear contractions on tcgen05 as 3xTF32 (error-compensated, fp32-equivalent) with fp32 TMEM accumulation")},
+                                "fp32 in/out; Linear contractions on wgmma as 3xTF32 (error-compensated, fp32-equivalent) with fp32 register accumulation")},
+            "device": {"name": props.name, "sms": props.multi_processor_count, "power_limit_w": power_limit(local)},
             "e2e": {"value": e2e, "unit": "queries/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4,
                     "ms_per_step": ms_e2e / args.steps, "epoch_loss": ep_loss_host},
             "gpu_launches": int(launches), "clocks": clk.summary(), "roofline": roof, "cpu_baseline": cpu,
@@ -431,7 +470,7 @@ def build_roofline(cfg, B, tm, steps_timed, ms_per_step):
     step_bytes = alg["bytes_per_query"] * B
     roof = {}
     traffic_tab = {}
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")       # dram bytes per launch from the committed ncu --set full captures
+    tpath = os.path.join(ROOT, "profiles", "traffic.json")       # optional: measured DRAM bytes per launch, by kernel name
     if os.path.exists(tpath):
         traffic_tab = json.load(open(tpath))
     if cfg["sf"]["sf_id"] == "pointsf":
@@ -497,7 +536,8 @@ def build_roofline(cfg, B, tm, steps_timed, ms_per_step):
         loss_k = [k for k in tm if k.startswith(("pairwise_bce", "approxndcg_kernel", "lambdaloss_kernel"))]
         if loss_k:
             lms = sum(tm[k][1] for k in loss_k) / steps_timed
-            mufu_peak = 16 * 148 * peaks["sm_max_mhz"] * 1e6          # MUFU results per second (16 / clk / SM)
+            sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+            mufu_peak = 16 * sms * peaks["sm_max_mhz"] * 1e6          # MUFU results per second (16 / clk / SM)
             pps = alg["pairs_per_query"] * B / (lms * 1e-3)
             roof["loss"] = {"kernel": loss_k[0], "ms_per_step": lms, "pairs_per_s": pps,
                             "mufu_ops_per_pair": 4, "mufu_frac": 4 * pps / mufu_peak,
@@ -510,7 +550,7 @@ def build_roofline(cfg, B, tm, steps_timed, ms_per_step):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=100)
+    ap.add_argument("--steps", type=int, default=None, help="timed steps (default: 100; configs c/d: 20/50)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference", "reference-cuda"])
     ap.add_argument("--config", default="b", choices=["a", "b", "c", "d", "e"], help="BASELINE.json configs[0..4]")
@@ -519,11 +559,15 @@ def main():
     ap.add_argument("--docs", type=int, default=256, help="config e: documents per query (32..1024)")
     ap.add_argument("--enc-layers", type=int, default=6, help="config c: encoder layers (6 = code default, 3 = test JSON)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's loss and updated parameters as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     cfg = make_config(args)
-    if args.config != "b" and args.steps == 100:
-        args.steps = {"a": 100, "c": 20, "d": 50, "e": 100}[args.config]
+    if args.steps is None:
+        args.steps = {"a": 100, "b": 100, "c": 20, "d": 50, "e": 100}[args.config]
+    if args.steps < 1:
+        raise SystemExit("--steps must be >= 1")
     if args.impl == "reference":
         run_reference(args, cfg, "cpu")
     elif args.impl == "reference-cuda":

@@ -1,4 +1,4 @@
-/* ptranking_b200.h -- C ABI of the B200-native PTRanking hot path (libptranking_b200.so).
+/* ptranking_b200.h -- C ABI of the H100-native PTRanking hot path (libptranking_b200.so).
  *
  * PTRanking has no FFI of its own: its plugin API is a Python class contract
  * (SURVEY.md 8b).  This header is the boundary a maintainer binds from that
@@ -182,11 +182,11 @@ int ptrb200_standard_scale(const float* X, const int32_t* offsets, float* out, i
 #define PTRB200_NORM_BN2  2   /* LTRBatchNorm2: statistics per query */
 
 #define PTRB200_MATH_SIMT   0   /* fp32 FMA on the SIMT pipes (any shape)                              */
-#define PTRB200_MATH_3XTF32 1   /* tcgen05 kind::tf32, error-compensated 3-pass split: fp32-equivalent */
-#define PTRB200_MATH_TF32   2   /* tcgen05 kind::tf32, single pass (10-bit mantissa operands)           */
+#define PTRB200_MATH_3XTF32 1   /* wgmma tf32, error-compensated 3-pass split: fp32-equivalent     */
+#define PTRB200_MATH_TF32   2   /* wgmma tf32, single pass (10-bit mantissa operands)               */
 #define PTRB200_MATH_BF16   3   /* every GEMM operand (features, activations, weights, gradients) rounded to bf16
                                    (round-to-nearest-even), products exact, fp32 accumulation: the numerics of a bf16
-                                   tensor-core GEMM, issued as one kind::tf32 pass (bf16 values are tf32 values);
+                                   tensor-core GEMM, issued as one tf32 wgmma pass (bf16 values are tf32 values);
                                    tensors stay fp32 in memory.  Needs tensor-core-eligible widths (no SIMT fallback) */
 
 typedef struct ptrb200_ffnet {
@@ -329,7 +329,7 @@ int ptrb200_attention_bwd(const float* Q, const float* K, const float* V, const 
                           int B, int n, int H, int D, float dropout_p, uint64_t seed, uint64_t offset,
                           ptrb200_stream_t stream);
 /* Tensor-core variant of the two calls above (same maths, same dropout stream): every contraction is a batched
- * tcgen05 kind::tf32 GEMM (passes = 3: 3xTF32 split, fp32-grade; 1: plain TF32); the attention matrix
+ * wgmma tf32 GEMM (passes = 3: 3xTF32 split, fp32-grade; 1: plain TF32); the attention matrix
  * P[B*H,n,n] is materialised in HBM and kept for the backward pass.
  * scratch: ptrb200_attention_tc_workspace_floats(B,n,H,D,backward) floats. */
 int64_t ptrb200_attention_tc_workspace_floats(int B, int n, int H, int D, int backward);
@@ -380,7 +380,7 @@ int ptrb200_elementwise(int op, const float* a, const float* b, float* out, int6
                         float dropout_p, uint64_t seed, uint64_t offset, ptrb200_stream_t stream);
 
 /* ---- tensor-core GEMM building block ---------------------------------------------------- */
-/* C[M,N] = A[M,K] * B[N,K]^T in fp32 through tcgen05.mma kind::tf32 with TMEM accumulation
+/* C[M,N] = A[M,K] * B[N,K]^T in fp32 through tf32 wgmma with register accumulation
  * (the contraction of nn.Linear: torch.nn.functional.linear as called by every ff_* layer of
  * get_stacked_FFNet, ptranking/base/utils.py:302,320).  passes = 1: plain TF32 operands;
  * passes = 3: error-compensated 3xTF32 (fp32-equivalent accuracy).  N <= 256. */
@@ -388,7 +388,7 @@ int ptrb200_tc_gemm_nt(const float* A, const float* B, float* C, int M, int N, i
                        ptrb200_stream_t stream);
 
 /* dW[N,K] = dZ[rows,N]^T * P[rows,K] (the weight gradient autograd forms for nn.Linear) with both operands
- * consumed MN-major by tcgen05.mma; partials: 296*N*K floats of scratch.  N <= 128, K <= 256, K % 4 == 0. */
+ * transposed into K-major wgmma operands; partials: 296*N*K floats of scratch.  N <= 128, K <= 256, K % 4 == 0. */
 int ptrb200_tc_wgrad(const float* dZ, const float* P, float* dW, float* partials, int rows, int N, int K, int passes,
                      ptrb200_stream_t stream);
 

@@ -1,11 +1,11 @@
-"""ptranking_b200 -- B200-native (sm_100a) scoring-and-loss hot path behind PTRanking's plugin API.
+"""ptranking_b200 -- H100-native (sm_90a) scoring-and-loss hot path behind PTRanking's plugin API.
 
     import ptranking_b200
     ptranking_b200.install()           # swap the loss classes into ptranking.ltr_adhoc.eval.ltr
     LTREvaluator(cuda=0).run(model_id='LambdaRank', ...)   # the unmodified reference driver
 
 Importing the package never touches the GPU; the first kernel call loads
-lib/libptranking_b200.so and raises if it (or an sm_100 device) is missing.
+lib/libptranking_b200.so and raises if it (or an sm_90 device) is missing.
 """
 from .ltr_adhoc.pairwise.ranknet import RankNet
 from .ltr_adhoc.listwise.lambdarank import LambdaRank
@@ -25,7 +25,7 @@ __version__ = "0.1.0"
 
 
 def install(module=None):
-    """Register the B200 classes where the reference resolves model ids by name:
+    """Register the CUDA classes where the reference resolves model ids by name:
     ``globals()[model_id]`` in ptranking/ltr_adhoc/eval/ltr.py:166-171."""
     if module is None:
         import ptranking.ltr_adhoc.eval.ltr as module  # the reference package must be importable

@@ -1,7 +1,7 @@
 """ctypes binding of libptranking_b200.so (the C ABI declared in include/ptranking_b200.h).
 
 There is no CPU fallback: if the shared library is missing or the device is not
-sm_100, loading raises -- the product path never routes around the CUDA kernels.
+sm_90, loading raises -- the product path never routes around the CUDA kernels.
 """
 from __future__ import annotations
 
@@ -167,7 +167,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: build it with `python -m ptranking_b200.build` "
-            "(nvcc, sm_100a).  ptranking_b200 has no CPU or PyTorch fallback.")
+            "(nvcc, sm_90a).  ptranking_b200 has no CPU or PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)          # AttributeError here = header/library mismatch

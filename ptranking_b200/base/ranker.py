@@ -1,5 +1,5 @@
 """NeuralRanker / Evaluator with the reference's method set (ptranking/base/ranker.py:28-65,
-:67-95, :189-200, :479-630) driving the B200 kernels.
+:67-95, :189-200, :479-630) driving the CUDA kernels.
 
 Differences kept deliberately small and listed in DESIGN.md: tensors live on the CUDA
 device for the whole step; nDCG is computed by the in-CTA sort kernel on the device

@@ -46,7 +46,7 @@ class StackedFFNet(nn.Module):
     def __init__(self, ff_dims, AF=None, TL_AF=None, apply_tl_af=False, dropout=0.1,
                  BN=True, bn_type=None, bn_affine=False, device=None, math_mode=None):
         super().__init__()
-        # "3xtf32" (default): tcgen05 tensor cores with the fp32-equivalent 3-pass TF32 split;
+        # "3xtf32" (default): wgmma tensor cores with the fp32-equivalent 3-pass TF32 split;
         # "tf32": single pass; "simt": fp32 FMA kernels (also the fallback for widths the MMA tiles reject)
         math_mode = math_mode or os.environ.get("PTRANKING_B200_MATH", "3xtf32")
         assert ff_dims is not None and len(ff_dims) >= 2

@@ -1,9 +1,9 @@
-"""Build recipe for libptranking_b200.so (sm_100a only, in-tree).
+"""Build recipe for libptranking_b200.so (sm_90a only, in-tree).
 
     python -m ptranking_b200.build          # rebuild if any source is newer than the .so
     python -m ptranking_b200.build --force
 
-nvcc cross-compiles without a GPU; the .so is git-ignored but travels to the GPU box.
+nvcc cross-compiles without a GPU; the .so and its objects are build products (git-ignored).
 """
 from __future__ import annotations
 
@@ -20,7 +20,7 @@ LIB = os.path.join(LIB_DIR, "libptranking_b200.so")
 HEADER = os.path.join(os.path.dirname(PKG), "include", "ptranking_b200.h")
 
 NVCC_FLAGS = [
-    "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr",
     "-Xptxas", "-v",
 ]
@@ -62,7 +62,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         log.append(f"== {os.path.basename(src)}\n{out}")
         if pr.returncode != 0:
             raise RuntimeError(f"nvcc failed on {src}:\n{out}")
-    link = [_nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB, *objs,
+    link = [_nvcc(), "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB, *objs,
             "-Xcompiler", "-fPIC", "-lcuda"]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:

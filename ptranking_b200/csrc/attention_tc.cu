@@ -1,20 +1,19 @@
-// attention_tc.cu -- multi-head self-attention with every contraction on tcgen05 tensor cores.
+// attention_tc.cu -- multi-head self-attention with every contraction on wgmma tensor cores.
 //
 // MultiheadAttention.forward, ptranking/base/list_ranker.py:226-248:
 //     S = Q K^T / sqrt(d)   ->   A = softmax(S)   ->   A_d = dropout(A)   ->   O = A_d V
 // and its autograd.  "Materialised S" design: the six contractions of forward + backward
 //     S = Q K^T,   O = A_d V,   dA_d = dO V^T,   dQ = dS K,   dK = dS^T Q,   dV = A_d^T dO
-// all run through a batched, strided  C[z] = alpha * op(A[z]) * B[z]^T  kernel (kind::tf32, 3xTF32 split, fp32
-// accumulation in TMEM); row softmax / softmax-backward are streaming SIMT kernels over the [n,n] score tensor.  A factor that
-// enters a contraction transposed (V, K, Q, dO as [key|query, d]; dS and A_d as [query, key] for dK / dV) is consumed in place
-// as an MN-major tcgen05 operand, never transposed in memory.  The [n,n] tensors live in HBM (n <= 1024 per
-// list: 134 MB per layer at B=64, n=512, 2 heads).
+// all run through a batched, strided  C[z] = alpha * op(A[z]) * B[z]^T  kernel (tf32 wgmma, 3xTF32 split, fp32
+// accumulation in registers); row softmax / softmax-backward are streaming SIMT kernels over the [n,n] score tensor.  A factor
+// that enters a contraction transposed (V, K, Q, dO as [key|query, d]; dS and A_d as [query, key] for dK / dV) is read in
+// place with coalesced loads and transposed on its way into shared memory (wgmma takes 32-bit operands K-major only), never
+// transposed in HBM.  The [n,n] tensors live in HBM (n <= 1024 per list: 134 MB per layer at B=64, n=512, 2 heads).
 // Two kernels implement the batched GEMM: bgemm_nt_tc_kernel takes any shape; bgemm_fast_kernel (every extent, pitch and
 // base address a multiple of four floats -- the attention core's own shapes) has the operand layouts and the dropout view
 // as template parameters, loads one K-chunk ahead and writes full-width tiles through shared memory; both produce the
 // same bits.  The row-pitched entry points (_ld) read Q|K|V side by side from one projection output and take per-query key
-// counts for padded ragged batches.  A version that kept the score tile in TMEM across QK^T and the softmax was built,
-// measured slower (one CTA per SM, strictly serial phases) and removed: DESIGN.md 4.
+// counts for padded ragged batches.
 #include "common.cuh"
 #include "tc.cuh"
 
@@ -33,12 +32,46 @@ struct BGemmArgs {
     int drop_mode;
     DropCfg drop;
     // operand storage: 0 = K-major as written above (A[M,K], B[N,K] row-major); 1 = MN-major, the operand is stored
-    // transposed ([K,M] resp. [K,N] row-major, pitch lda/ldb between k-rows) and consumed as an MN-major tcgen05 operand
-    // (SWIZZLE_128B_BASE32B), so a transposed factor never has to be materialised.  drop_mode 2 goes with a_mn.
+    // transposed ([K,M] resp. [K,N] row-major, pitch lda/ldb between k-rows) and transposed while it is staged, so a
+    // transposed factor never has to be materialised in HBM.  drop_mode 2 goes with a_mn.
     int a_mn, b_mn;
 };
 
-constexpr int BG_THREADS = 256, BG_NT = 128;
+constexpr int BG_THREADS = 256, BG_NT = 128;      // two warpgroups, 64 rows of the 128 x 128 tile each
+
+// store 4 consecutive M (or N) elements of one k-row of an MN-major source into the K-major operand image
+static __device__ __forceinline__ void store_mn4(unsigned char* buf, int r, int k, float4 v) {
+    *reinterpret_cast<float*>(buf + tc::swz_elem(r, k)) = v.x;
+    *reinterpret_cast<float*>(buf + tc::swz_elem(r + 1, k)) = v.y;
+    *reinterpret_cast<float*>(buf + tc::swz_elem(r + 2, k)) = v.z;
+    *reinterpret_cast<float*>(buf + tc::swz_elem(r + 3, k)) = v.w;
+}
+static __device__ __forceinline__ void store_op(unsigned char* buf, bool mn, uint32_t off_k, int r_mn, int k_mn, float4 v) {
+    if (mn) store_mn4(buf, r_mn, k_mn, v);
+    else *reinterpret_cast<float4*>(buf + off_k) = v;
+}
+
+// the four K-steps of one 32-column chunk (columns beyond K are staged as zeros): warpgroup wg multiplies A rows
+// [64 wg, +64) by all NPc columns of B.  3xTF32: the small a_lo*b_hi + a_hi*b_lo terms accumulate apart from the main
+// products (the epilogue adds them), so two thirds of the accumulate steps leave the main chain.
+template <int PASSES, int NPc>
+static __device__ __forceinline__ void bg_mma_chunk(float (&acc)[NPc / 2], float (&cor)[NPc / 2], const unsigned char* a_hi,
+                                                    const unsigned char* b_hi, int wg) {
+    const uint32_t a_s = tc::smem_u32(a_hi) + wg * 8192, b_s = tc::smem_u32(b_hi);
+    const uint64_t ah = tc::smem_desc_sw128(a_s, 1024), al = tc::smem_desc_sw128(a_s + 16384, 1024);
+    const uint64_t bh = tc::smem_desc_sw128(b_s, 1024), bl = tc::smem_desc_sw128(b_s + 16384, 1024);
+    tc::wg_fence();
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+        if (PASSES == 3) {
+            tc::mma_tf32<NPc>(cor, al + 2 * s, bh + 2 * s, 1u);
+            tc::mma_tf32<NPc>(cor, ah + 2 * s, bl + 2 * s, 1u);
+        }
+        tc::mma_tf32<NPc>(acc, ah + 2 * s, bh + 2 * s, 1u);
+    }
+    tc::wg_commit();
+    tc::wg_wait<0>();                 // the same threads stage the next chunk
+}
 
 template <int PASSES>
 __global__ void __launch_bounds__(BG_THREADS) bgemm_nt_tc_kernel(BGemmArgs g) {
@@ -48,10 +81,8 @@ __global__ void __launch_bounds__(BG_THREADS) bgemm_nt_tc_kernel(BGemmArgs g) {
     unsigned char* a_lo = a_hi + 16384;
     unsigned char* b_hi = a_lo + 16384;
     unsigned char* b_lo = b_hi + 16384;
-    uint64_t* mbar = reinterpret_cast<uint64_t*>(b_lo + 16384);
-    uint32_t* slot = reinterpret_cast<uint32_t*>(mbar + 1);
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, wg = tid >> 7;
     const int z = blockIdx.z, zb = z / g.H, zh = z % g.H;
     const float* A = g.A + zb * g.sAb + zh * g.sAh;
     const float* B = g.B + zb * g.sBb + zh * g.sBh;
@@ -60,20 +91,6 @@ __global__ void __launch_bounds__(BG_THREADS) bgemm_nt_tc_kernel(BGemmArgs g) {
     const int N = min(BG_NT, g.N - n0), NP = ((N + 15) / 16) * 16;
     const int K = g.K;
     const int nchunks = (K + 31) / 32;
-    // The tensor core accumulates with truncation, a bias that grows linearly with the number of accumulation steps.
-    // Long contractions therefore alternate between two main accumulators, and the small a_lo*b_hi + a_hi*b_lo correction
-    // terms get an accumulator of their own; the epilogue adds them up in round-to-nearest fp32.
-    const int nmain = (nchunks > 4 && 3 * NP <= 256) ? 2 : 1;
-    const int nacc = nmain + (PASSES == 3 ? 1 : 0);
-    const uint32_t need = (uint32_t)(nacc * NP);
-    const uint32_t tmem_cols = need <= 32 ? 32 : need <= 64 ? 64 : need <= 128 ? 128 : 256;
-    if (tid == 0) { tc::mbar_init(mbar, 1); tc::mbar_fence_init(); }
-    if (warp == 0) tc::tmem_alloc(slot, tmem_cols);
-    tc::fence_before_sync();
-    __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tmem = *slot;
-    const uint32_t idesc = tc::instr_desc(2, 128, NP) | (g.a_mn ? (1u << 15) : 0u) | (g.b_mn ? (1u << 16) : 0u);
     const bool vecA = (g.lda & 3) == 0 && ((reinterpret_cast<uintptr_t>(A) & 15) == 0);
     const bool vecB = (g.ldb & 3) == 0 && ((reinterpret_cast<uintptr_t>(B) & 15) == 0);
 
@@ -95,6 +112,11 @@ __global__ void __launch_bounds__(BG_THREADS) bgemm_nt_tc_kernel(BGemmArgs g) {
         if (c0 + 3 < lim) v.w = p[c0 + 3];
         return v;
     };
+    tc::with_width(NP, [&](auto W) {
+    constexpr int NPc = decltype(W)::value;
+    float acc[NPc / 2], cor[NPc / 2];
+#pragma unroll
+    for (int e = 0; e < NPc / 2; ++e) { acc[e] = 0.0f; cor[e] = 0.0f; }
     for (int c = 0; c < nchunks; ++c) {
         const int k0 = c * 32;
         float4 av[4], bv[4];
@@ -107,13 +129,12 @@ __global__ void __launch_bounds__(BG_THREADS) bgemm_nt_tc_kernel(BGemmArgs g) {
             if (g.b_mn) bv[i] = (k0 + kr < K) ? load4m(B + (size_t)(k0 + kr) * g.ldb, n0 + mu, n0 + N, vecB) : make_float4(0.f, 0.f, 0.f, 0.f);
             else bv[i] = (r < N) ? load4(B + (size_t)(n0 + r) * g.ldb, k, vecB) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
-        if (c > 0) tc::mbar_wait(mbar, (c - 1) & 1);
+        if (c > 0) __syncthreads();                           // both warpgroups' MMAs of chunk c-1 are done with the operand buffers
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             const int u = tid + i * BG_THREADS, r = u >> 3, j = u & 7, k = k0 + j * 4;
             const int kr = u >> 5, mu = (u & 31) * 4;
             const uint32_t off_k = tc::swz_offset(r, j);                                             // K-major slot
-            const uint32_t off_mn = (uint32_t)((u & 31) >> 3) * 4096u + tc::swz32_offset(kr, u & 7);   // MN-major: 32-column chunk, k-row, unit
             float4 v = av[i];
             if (g.drop_mode && g.drop.thr) {
                 float* e = &v.x;
@@ -127,75 +148,30 @@ __global__ void __launch_bounds__(BG_THREADS) bgemm_nt_tc_kernel(BGemmArgs g) {
             }
             float4 h, l;
             tc::split_tf32_rn(v.x, h.x, l.x); tc::split_tf32_rn(v.y, h.y, l.y); tc::split_tf32_rn(v.z, h.z, l.z); tc::split_tf32_rn(v.w, h.w, l.w);
-            const uint32_t offa = g.a_mn ? off_mn : off_k;
-            *reinterpret_cast<float4*>(a_hi + offa) = PASSES == 3 ? h : v;
-            if (PASSES == 3) *reinterpret_cast<float4*>(a_lo + offa) = l;
+            store_op(a_hi, g.a_mn, off_k, mu, kr, PASSES == 3 ? h : v);
+            if (PASSES == 3) store_op(a_lo, g.a_mn, off_k, mu, kr, l);
             const float4 w = bv[i];
             tc::split_tf32_rn(w.x, h.x, l.x); tc::split_tf32_rn(w.y, h.y, l.y); tc::split_tf32_rn(w.z, h.z, l.z); tc::split_tf32_rn(w.w, h.w, l.w);
-            const uint32_t offb = g.b_mn ? off_mn : off_k;
-            *reinterpret_cast<float4*>(b_hi + offb) = PASSES == 3 ? h : w;
-            if (PASSES == 3) *reinterpret_cast<float4*>(b_lo + offb) = l;
+            store_op(b_hi, g.b_mn, off_k, mu, kr, PASSES == 3 ? h : w);
+            if (PASSES == 3) store_op(b_lo, g.b_mn, off_k, mu, kr, l);
         }
         tc::fence_proxy_async();
         __syncthreads();
-        if (warp == 0) {
-            tc::fence_after_sync();
-            const int ksteps = min(4, (K - k0 + 7) / 8);
-            // K-major: 8-row atoms 1024 B apart, +32 B per K-step; MN-major: 32-column chunks 4096 B apart, 4-row groups 512 B
-            // apart, +1024 B per K-step (descriptor addresses count 16-byte units)
-            uint64_t ah = g.a_mn ? tc::smem_desc_sw128_mn(tc::smem_u32(a_hi), 4096, 512) : tc::smem_desc_sw128(tc::smem_u32(a_hi), 1024);
-            uint64_t al = g.a_mn ? tc::smem_desc_sw128_mn(tc::smem_u32(a_lo), 4096, 512) : tc::smem_desc_sw128(tc::smem_u32(a_lo), 1024);
-            uint64_t bh = g.b_mn ? tc::smem_desc_sw128_mn(tc::smem_u32(b_hi), 4096, 512) : tc::smem_desc_sw128(tc::smem_u32(b_hi), 1024);
-            uint64_t bl = g.b_mn ? tc::smem_desc_sw128_mn(tc::smem_u32(b_lo), 4096, 512) : tc::smem_desc_sw128(tc::smem_u32(b_lo), 1024);
-            const uint64_t da = g.a_mn ? 64 : 2, db = g.b_mn ? 64 : 2;
-            if (tc::elect_one()) {
-                const uint32_t t_main = tmem + (uint32_t)((c % nmain) * NP), t_corr = tmem + (uint32_t)(nmain * NP);
-                for (int s = 0; s < ksteps; ++s) {
-                    const uint32_t acc_m = (c < nmain && s == 0) ? 0u : 1u;
-                    if (PASSES == 3) {
-                        tc::mma_tf32(t_corr, al, bh, idesc, (c == 0 && s == 0) ? 0u : 1u);
-                        tc::mma_tf32(t_corr, ah, bl, idesc, 1u);
-                    }
-                    tc::mma_tf32(t_main, ah, bh, idesc, acc_m);
-                    ah += da; al += da; bh += db; bl += db;
-                }
-                tc::mma_commit(mbar);
-            }
-            __syncwarp();
-        }
+        bg_mma_chunk<PASSES, NPc>(acc, cor, a_hi, b_hi, wg);
     }
-    tc::mbar_wait(mbar, (nchunks - 1) & 1);
-    tc::fence_after_sync();
-    {   // epilogue: TMEM lane = row; warps (q, half) split the columns
-        const int q = warp & 3, half = warp >> 2;
-        const int row = m0 + q * 32 + lane;
-        const int cols_half = ((NP / 8 + 1) / 2) * 8;
-        const int c_begin = half == 0 ? 0 : cols_half, c_end = half == 0 ? min(cols_half, NP) : NP;
-        float* crow = C + (size_t)min(row, g.M - 1) * g.ldc + n0;
+    {   // epilogue: registers -> C
         const bool vecC = (g.ldc & 3) == 0 && ((reinterpret_cast<uintptr_t>(C + n0) & 15) == 0);
-        for (int c0 = c_begin; c0 < c_end; c0 += 8) {
-            float v[8];
-            tc::tmem_ld8(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-            for (int a = 1; a < nacc; ++a) {
-                float w[8];
-                tc::tmem_ld8(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * NP + c0), w);
 #pragma unroll
-                for (int e = 0; e < 8; ++e) v[e] += w[e];
-            }
-            if (row < g.M && c0 < N) {
-                if (c0 + 8 <= N && vecC) {
-                    *reinterpret_cast<float4*>(crow + c0) = make_float4(v[0] * g.alpha, v[1] * g.alpha, v[2] * g.alpha, v[3] * g.alpha);
-                    *reinterpret_cast<float4*>(crow + c0 + 4) = make_float4(v[4] * g.alpha, v[5] * g.alpha, v[6] * g.alpha, v[7] * g.alpha);
-                } else {
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) if (c0 + e < N) crow[c0 + e] = v[e] * g.alpha;
-                }
-            }
+        for (int e = 0; e < NPc / 2; e += 2) {
+            const int row = m0 + wg * 64 + tc::acc_row(e), col = tc::acc_col(e);
+            if (row >= g.M || col >= N) continue;
+            const float v0 = (acc[e] + cor[e]) * g.alpha, v1 = (acc[e + 1] + cor[e + 1]) * g.alpha;
+            float* p = C + (size_t)row * g.ldc + n0 + col;
+            if (col + 1 < N && vecC) *reinterpret_cast<float2*>(p) = make_float2(v0, v1);
+            else { p[0] = v0; if (col + 1 < N) p[1] = v1; }
         }
     }
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tmem, tmem_cols);
+    });
 }
 
 // Alignment-specialised variant of the kernel above: same tiling, same accumulators, same results bit for bit (identical
@@ -206,18 +182,15 @@ __global__ void __launch_bounds__(BG_THREADS) bgemm_nt_tc_kernel(BGemmArgs g) {
 // cannot assume quad alignment); B units beyond the padded tile width are never touched.  The attention core's six
 // contractions all qualify; odd shapes keep the general kernel.
 template <int PASSES, int A_MN, int B_MN, int DROP>
-__global__ void __launch_bounds__(BG_THREADS, 2) bgemm_fast_kernel(BGemmArgs g) {
+__global__ void __launch_bounds__(BG_THREADS, 1) bgemm_fast_kernel(BGemmArgs g) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     unsigned char* a_hi = base;
     unsigned char* a_lo = a_hi + 16384;
     unsigned char* b_hi = a_lo + 16384;
     unsigned char* b_lo = b_hi + 16384;
-    uint64_t* mbar = reinterpret_cast<uint64_t*>(base + 128 * (BG_NT + 4) * 4);     // beyond the epilogue's staging tile, which overlays the operands
-    (void)b_lo;
-    uint32_t* slot = reinterpret_cast<uint32_t*>(mbar + 1);
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
     const int z = blockIdx.z, zb = z / g.H, zh = z % g.H;
     const float* A = g.A + zb * g.sAb + zh * g.sAh;
     const float* B = g.B + zb * g.sBb + zh * g.sBh;
@@ -226,28 +199,16 @@ __global__ void __launch_bounds__(BG_THREADS, 2) bgemm_fast_kernel(BGemmArgs g) 
     const int N = min(BG_NT, g.N - n0), NP = ((N + 15) / 16) * 16;
     const int K = g.K;
     const int nchunks = (K + 31) / 32;
-    const int nmain = (nchunks > 4 && 3 * NP <= 256) ? 2 : 1;
-    const int nacc = nmain + (PASSES == 3 ? 1 : 0);
-    const uint32_t need = (uint32_t)(nacc * NP);
-    const uint32_t tmem_cols = need <= 32 ? 32 : need <= 64 ? 64 : need <= 128 ? 128 : 256;
-    if (tid == 0) { tc::mbar_init(mbar, 1); tc::mbar_fence_init(); }
-    if (warp == 0) tc::tmem_alloc(slot, tmem_cols);
-    tc::fence_before_sync();
-    __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tmem = *slot;
-    const uint32_t idesc = tc::instr_desc(2, 128, NP) | (A_MN ? (1u << 15) : 0u) | (B_MN ? (1u << 16) : 0u);
 
     // ---- chunk-invariant geometry of this thread's units (unit index i = 0..3) ----
     const int jk = tid & 7, rk = tid >> 3;            // K-major: 16-byte unit jk of row rk + 32 i
     const int cm = (tid & 31) * 4, km = tid >> 5;     // MN-major: columns cm..cm+3 of k-row km + 8 i
     const float* pa; const float* pb;
     size_t sa, sb;                                    // pointer step per unit index
-    uint32_t oa, ob;                                  // swizzled offset of unit 0 (+4096 resp. +1024 per unit index)
+    uint32_t oa = 0, ob = 0;                          // K-major: swizzled offset of unit 0 (+4096 per unit index)
     uint32_t am = 0, bm = 0;                          // bit i: unit i lies inside the tile along M / N (bit 4+i: and is staged at all)
     if (A_MN) {
         pa = A + (size_t)km * g.lda + m0 + cm; sa = (size_t)8 * g.lda;
-        oa = (uint32_t)(cm >> 5) * 4096u + tc::swz32_offset(km, jk);
         am = (m0 + cm < g.M) ? 0xfu : 0u;
     } else {
         pa = A + (size_t)(m0 + rk) * g.lda + jk * 4; sa = (size_t)32 * g.lda;
@@ -257,7 +218,6 @@ __global__ void __launch_bounds__(BG_THREADS, 2) bgemm_fast_kernel(BGemmArgs g) 
     }
     if (B_MN) {
         pb = B + (size_t)km * g.ldb + n0 + cm; sb = (size_t)8 * g.ldb;
-        ob = (uint32_t)(cm >> 5) * 4096u + tc::swz32_offset(km, jk);
         bm = (cm < N ? 0xfu : 0u) | (cm < NP ? 0xf0u : 0u);
     } else {
         pb = B + (size_t)(n0 + rk) * g.ldb + jk * 4; sb = (size_t)32 * g.ldb;
@@ -265,7 +225,11 @@ __global__ void __launch_bounds__(BG_THREADS, 2) bgemm_fast_kernel(BGemmArgs g) 
 #pragma unroll
         for (int i = 0; i < 4; ++i) bm |= (rk + 32 * i < N ? (1u << i) : 0u) | (rk + 32 * i < NP ? (16u << i) : 0u);
     }
-    constexpr uint32_t OA_STEP = A_MN ? 1024u : 4096u, OB_STEP = B_MN ? 1024u : 4096u;
+    // MN-major units are transposed into the K-major image: 4 elements (rows cm..cm+3) of k-row km + 8 i
+    auto put = [&](unsigned char* buf, bool mn, uint32_t off, int i, float4 v) {
+        if (mn) store_mn4(buf, cm, km + 8 * i, v);
+        else *reinterpret_cast<float4*>(buf + off + i * 4096u) = v;
+    };
     // dropout counter: key + GOLD * quad, quad = element id / 4 of the unit's first element (ids as in the general kernel)
     constexpr uint64_t GOLD = 0x9e3779b97f4a7c15ull;
     uint64_t dctr = 0, dstep_i = 0, dstep_c = 0;
@@ -294,13 +258,18 @@ __global__ void __launch_bounds__(BG_THREADS, 2) bgemm_fast_kernel(BGemmArgs g) 
         pa += A_MN ? (size_t)32 * g.lda : 32; pb += B_MN ? (size_t)32 * g.ldb : 32;
     };
     load_chunk(0);
+    tc::with_width(NP, [&](auto W) {
+    constexpr int NPc = decltype(W)::value;
+    float acc[NPc / 2], cor[NPc / 2];
+#pragma unroll
+    for (int e = 0; e < NPc / 2; ++e) { acc[e] = 0.0f; cor[e] = 0.0f; }
     for (int c = 0; c < nchunks; ++c) {
         const int k0 = c * 32;
         float4 av[4], bv[4];
 #pragma unroll
         for (int i = 0; i < 4; ++i) { av[i] = nav[i]; bv[i] = nbv[i]; }
         if (c + 1 < nchunks) load_chunk(c + 1);
-        if (c > 0) tc::mbar_wait(mbar, (c - 1) & 1);
+        if (c > 0) __syncthreads();                           // both warpgroups' MMAs of chunk c-1 are done with the operand buffers
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             float4 v = av[i];
@@ -313,94 +282,47 @@ __global__ void __launch_bounds__(BG_THREADS, 2) bgemm_fast_kernel(BGemmArgs g) 
             }
             float4 h, l;
             tc::split_tf32_rn(v.x, h.x, l.x); tc::split_tf32_rn(v.y, h.y, l.y); tc::split_tf32_rn(v.z, h.z, l.z); tc::split_tf32_rn(v.w, h.w, l.w);
-            *reinterpret_cast<float4*>(a_hi + oa + i * OA_STEP) = PASSES == 3 ? h : v;
-            if (PASSES == 3) *reinterpret_cast<float4*>(a_lo + oa + i * OA_STEP) = l;
+            put(a_hi, A_MN, oa, i, PASSES == 3 ? h : v);
+            if (PASSES == 3) put(a_lo, A_MN, oa, i, l);
             if ((bm >> (4 + i)) & 1u) {
                 const float4 w = bv[i];
                 tc::split_tf32_rn(w.x, h.x, l.x); tc::split_tf32_rn(w.y, h.y, l.y); tc::split_tf32_rn(w.z, h.z, l.z); tc::split_tf32_rn(w.w, h.w, l.w);
-                *reinterpret_cast<float4*>(b_hi + ob + i * OB_STEP) = PASSES == 3 ? h : w;
-                if (PASSES == 3) *reinterpret_cast<float4*>(b_lo + ob + i * OB_STEP) = l;
+                put(b_hi, B_MN, ob, i, PASSES == 3 ? h : w);
+                if (PASSES == 3) put(b_lo, B_MN, ob, i, l);
             }
         }
         dctr += dstep_c;
         tc::fence_proxy_async();
         __syncthreads();
-        if (warp == 0) {
-            tc::fence_after_sync();
-            const int ksteps = min(4, (K - k0 + 7) / 8);
-            uint64_t ah = A_MN ? tc::smem_desc_sw128_mn(tc::smem_u32(a_hi), 4096, 512) : tc::smem_desc_sw128(tc::smem_u32(a_hi), 1024);
-            uint64_t al = A_MN ? tc::smem_desc_sw128_mn(tc::smem_u32(a_lo), 4096, 512) : tc::smem_desc_sw128(tc::smem_u32(a_lo), 1024);
-            uint64_t bh = B_MN ? tc::smem_desc_sw128_mn(tc::smem_u32(b_hi), 4096, 512) : tc::smem_desc_sw128(tc::smem_u32(b_hi), 1024);
-            uint64_t bl = B_MN ? tc::smem_desc_sw128_mn(tc::smem_u32(b_lo), 4096, 512) : tc::smem_desc_sw128(tc::smem_u32(b_lo), 1024);
-            constexpr uint64_t da = A_MN ? 64 : 2, db = B_MN ? 64 : 2;
-            if (tc::elect_one()) {
-                const uint32_t t_main = tmem + (uint32_t)((c % nmain) * NP), t_corr = tmem + (uint32_t)(nmain * NP);
-                for (int s = 0; s < ksteps; ++s) {
-                    const uint32_t acc_m = (c < nmain && s == 0) ? 0u : 1u;
-                    if (PASSES == 3) {
-                        tc::mma_tf32(t_corr, al, bh, idesc, (c == 0 && s == 0) ? 0u : 1u);
-                        tc::mma_tf32(t_corr, ah, bl, idesc, 1u);
-                    }
-                    tc::mma_tf32(t_main, ah, bh, idesc, acc_m);
-                    ah += da; al += da; bh += db; bl += db;
-                }
-                tc::mma_commit(mbar);
-            }
-            __syncwarp();
-        }
+        bg_mma_chunk<PASSES, NPc>(acc, cor, a_hi, b_hi, wg);
     }
-    tc::mbar_wait(mbar, (nchunks - 1) & 1);
-    tc::fence_after_sync();
-    const int q = warp & 3, half = warp >> 2;
     const float alpha = g.alpha;
     if (N == BG_NT) {
-        // full 128-column tile (the [n,n] score / dP tensors: the 134 MB outputs of the attention core).  TMEM lane = row, so a
-        // direct store has every lane of a warp writing into a different row (32-byte pieces of 32 rows per instruction);
-        // instead the tile goes through shared memory (the operand buffers are free: every MMA has completed) and leaves as
-        // whole 512-byte row segments, one row per warp instruction.
-        constexpr int PITCH = BG_NT + 4;                  // floats; 132 = 4 (mod 32): the row-strided float4 writes are conflict-free
+        // full 128-column tile (the [n,n] score / dP tensors: the 134 MB outputs of the attention core).  A thread's
+        // accumulators are 2-column pieces of 2 rows, so the tile goes through shared memory (the operand buffers are free:
+        // every MMA has completed) and leaves as whole 512-byte row segments, one row per warp instruction.
+        constexpr int PITCH = BG_NT + 4;                  // floats
         float* tile = reinterpret_cast<float*>(base);     // [128][PITCH] = 67,584 B (operands 65,536 B + the slack the host adds)
-        __syncthreads();                                  // (all threads are past their last operand stores; belt and braces)
-        for (int c0 = half * 64; c0 < half * 64 + 64; c0 += 8) {
-            float v[8];
-            tc::tmem_ld8(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-            for (int a = 1; a < nacc; ++a) {
-                float w[8];
-                tc::tmem_ld8(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * NP + c0), w);
+        __syncthreads();                                  // every warpgroup's MMAs have completed
 #pragma unroll
-                for (int e = 0; e < 8; ++e) v[e] += w[e];
-            }
-            float* t = tile + (q * 32 + lane) * PITCH + c0;
-            *reinterpret_cast<float4*>(t) = make_float4(v[0] * alpha, v[1] * alpha, v[2] * alpha, v[3] * alpha);
-            *reinterpret_cast<float4*>(t + 4) = make_float4(v[4] * alpha, v[5] * alpha, v[6] * alpha, v[7] * alpha);
+        for (int e = 0; e < NPc / 2; e += 2) {
+            const int r = wg * 64 + tc::acc_row(e), col = tc::acc_col(e);
+            *reinterpret_cast<float2*>(tile + r * PITCH + col) = make_float2((acc[e] + cor[e]) * alpha, (acc[e + 1] + cor[e + 1]) * alpha);
         }
         __syncthreads();
         const int rows_here = min(128, g.M - m0);
         for (int r = warp; r < rows_here; r += BG_THREADS / 32)
             *reinterpret_cast<float4*>(C + (size_t)(m0 + r) * g.ldc + n0 + lane * 4) = *reinterpret_cast<const float4*>(tile + r * PITCH + lane * 4);
-    } else {   // narrow tile: TMEM lane = row; warps (q, half) split the columns; every extent is a multiple of 4
-        const int row = m0 + q * 32 + lane;
-        const int cols_half = ((NP / 8 + 1) / 2) * 8;
-        const int c_begin = half == 0 ? 0 : cols_half, c_end = half == 0 ? min(cols_half, NP) : NP;
-        float* crow = C + (size_t)min(row, g.M - 1) * g.ldc + n0;
-        for (int c0 = c_begin; c0 < c_end; c0 += 8) {
-            float v[8];
-            tc::tmem_ld8(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-            for (int a = 1; a < nacc; ++a) {
-                float w[8];
-                tc::tmem_ld8(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * NP + c0), w);
+    } else {   // narrow tile: direct stores; every extent is a multiple of 4
 #pragma unroll
-                for (int e = 0; e < 8; ++e) v[e] += w[e];
-            }
-            if (row < g.M) {
-                if (c0 < N) *reinterpret_cast<float4*>(crow + c0) = make_float4(v[0] * alpha, v[1] * alpha, v[2] * alpha, v[3] * alpha);
-                if (c0 + 4 < N) *reinterpret_cast<float4*>(crow + c0 + 4) = make_float4(v[4] * alpha, v[5] * alpha, v[6] * alpha, v[7] * alpha);
-            }
+        for (int e = 0; e < NPc / 2; e += 2) {
+            const int row = m0 + wg * 64 + tc::acc_row(e), col = tc::acc_col(e);
+            if (row < g.M && col < N)
+                *reinterpret_cast<float2*>(C + (size_t)row * g.ldc + n0 + col) =
+                    make_float2((acc[e] + cor[e]) * alpha, (acc[e + 1] + cor[e + 1]) * alpha);
         }
     }
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tmem, tmem_cols);
+    });
 }
 
 // in-place row softmax over S[z][i][:] (one warp per row); also emits the per-row log-sum-exp.
@@ -458,7 +380,7 @@ static bool bgemm_general_forced() {
 }
 
 static int launch_bgemm(BGemmArgs& g, int Z, int passes, cudaStream_t st, const char* tag) {
-    const size_t smem = 1024 + 4 * 16384 + 64;
+    const size_t smem = 1024 + 4 * 16384;
     dim3 grid((g.M + 127) / 128, (g.N + BG_NT - 1) / BG_NT, Z);
     // the alignment-specialised kernel: every pitch, stride, extent and base address a multiple of four floats
     const auto q4 = [](long long v) { return (v & 3) == 0; };
@@ -468,7 +390,7 @@ static int launch_bgemm(BGemmArgs& g, int Z, int passes, cudaStream_t st, const 
                       (g.drop_mode == 0 || (g.drop_mode == 1 && !g.a_mn) || (g.drop_mode == 2 && g.a_mn));
     if (fast) {
         const int drop = g.drop.thr ? g.drop_mode : 0;
-        const size_t smem = 1024 + (size_t)128 * (BG_NT + 4) * 4 + 64;      // operands (64 KB) overlaid by the [128][132] output staging tile
+        const size_t smem = 1024 + (size_t)128 * (BG_NT + 4) * 4;      // operands (64 KB) overlaid by the [128][132] output staging tile
 #define PTRB200_BG_CASE(P, AM, BM, D) if ((passes == 3) == (P == 3) && g.a_mn == AM && g.b_mn == BM && drop == D) return launch_bgemm_fast<P, AM, BM, D>(g, grid, smem, st, tag);
         // the attention core's shapes (list_ranker.py:226-248 forward + autograd), 3xTF32 and single-pass
         PTRB200_BG_CASE(3, 0, 0, 0) PTRB200_BG_CASE(3, 0, 1, 0) PTRB200_BG_CASE(3, 0, 1, 1) PTRB200_BG_CASE(3, 1, 1, 0) PTRB200_BG_CASE(3, 1, 1, 2)

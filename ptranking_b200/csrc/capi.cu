@@ -96,8 +96,8 @@ int ptrb200_device_ok(void) {
         ptrb200::set_error("no CUDA device: %s", cudaGetErrorString(cudaGetLastError()));
         return 0;
     }
-    if (prop.major != 10) {
-        ptrb200::set_error("device %s is sm_%d%d; this library is built for sm_100a only", prop.name, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        ptrb200::set_error("device %s is sm_%d%d; this library is built for sm_90a only", prop.name, prop.major, prop.minor);
         return 0;
     }
     return 1;

@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for the sm_100a kernels of libptranking_b200.
+// common.cuh -- shared device helpers for the sm_90a kernels of libptranking_b200.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -18,6 +18,17 @@ int check_launch(const char* what);   // cudaGetLastError -> PTRB200_* code
 bool timing_enabled();
 void timing_before(const char* tag, cudaStream_t st);
 void timing_after(cudaStream_t st);
+
+// streaming multiprocessors of the current device (persistent grids launch one CTA per SM, grid-stride loops cap at a
+// multiple of it)
+static inline int num_sms() {
+    static int sms = 0;
+    if (!sms) {
+        int dev = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
+    }
+    return sms;
+}
 
 #define PTRB200_LAUNCH(kernel, grid, block, smem, stream, ...) \
     PTRB200_LAUNCH_TAG(#kernel, kernel, grid, block, smem, stream, __VA_ARGS__)

@@ -1,5 +1,5 @@
 // ffnet.cu -- stacked feed-forward scorer: Dropout -> Linear -> (BN | BN2) -> activation, repeated,
-// forward and backward, fp32 SIMT path (the tcgen05 path lives in gemm_tc.cu).
+// forward and backward, fp32 SIMT path (the tensor-core kernels live in ffnet_tc.cuh and gemm_tc.cu).
 //
 // Reference functions replaced (wildltr/ptranking @ f1d366c):
 //   get_stacked_FFNet            ptranking/base/utils.py:288-356
@@ -133,7 +133,7 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(GemmArgs g) {
 // sum partials[splits, count] over splits in fixed order -> out[count]
 // out[i] = sum_p partials[p][i].  Block = 64 outputs x 4 split groups: group q adds splits q, q+4, ... (independent
 // loads, unrolled), then the four group sums are combined in a fixed order -- deterministic, and 4x the loads in flight
-// of a one-thread-per-output loop over ~148 splits.
+// of a one-thread-per-output loop over one split per SM.
 __global__ void __launch_bounds__(256) reduce_splits_kernel(const float* __restrict__ partials, float* __restrict__ out, int splits, int count) {
     __shared__ float sh[4][64];
     const int e = threadIdx.x & 63, q = threadIdx.x >> 6;
@@ -221,8 +221,7 @@ __global__ void colstat_kernel(const float* __restrict__ Z, const float* __restr
 // product dA[r,c] = dropmask(dz[r] * w[c]) -- built on the fly here instead of being written and re-read.
 struct Rank1Src { const float* w; DropCfg drop; int round_bf16; };     // w == NULL: dA is a dense [rows, C] tensor
 
-// (4 resident CTAs per SM = 64 registers: measured best for this latency-bound sweep -- 0.51 ms per step against 0.58 at
-// 3 CTAs/72 registers and 0.62 at 5-6 CTAs with their spills)
+// (4 resident CTAs per SM = 64 registers: this sweep is latency-bound, so occupancy matters more than registers)
 // ACT >= 0 fixes the activation at compile time (the default scorer's GELU and ReLU): no per-element switch, and only the
 // derivative is evaluated.  ACT = -1 reads it from the NormRef.
 // PF: the loads of the NEXT row are issued before the current row is processed (the ncu capture of the dY sweep has 53 % of
@@ -631,7 +630,7 @@ struct LayerPlan {
     size_t ain_off;                              // tensor-core mode, l >= 1: the layer's rebuilt input dropout(act(norm(Z_{l-1}))) [rows,d_in]
 };
 struct Plan {
-    bool use_tc;                                 // every layer fits the tcgen05 kernels (else the SIMT path runs)
+    bool use_tc;                                 // every layer fits the tensor-core kernels (else the SIMT path runs)
     int passes;                                  // 3 = 3xTF32 (fp32-equivalent), 1 = TF32
     bool bf16;                                   // single pass with every operand rounded to bf16 first
     int tile_rows, seg_len, group_rows, tiles_per_group, ntiles, wg_grid, wg_rows;
@@ -645,15 +644,15 @@ struct Plan {
     size_t xpad_off, w0pad_off, dw0pad_off, dxpad_off;
 };
 
-// column blocking of the weight gradient: dZ columns in blocks of 128 (MMA M), input columns in blocks of <= 256 (MMA N)
+// column blocking of the weight gradient: dZ columns in blocks of 128 (two m64 MMA tiles), input columns in blocks of <= 256
 struct WgBlocks { int mblocks, kb, kblocks, gx; };
 static WgBlocks wgrad_blocks(int N, int K) {
     WgBlocks b;
     b.mblocks = (N + 127) / 128;
     b.kb = K <= 256 ? K : 256;
     b.kblocks = (K + b.kb - 1) / b.kb;
-    const int pairs = b.mblocks * b.kblocks;
-    b.gx = pairs == 1 ? 148 : (148 / pairs < 8 ? 8 : 148 / pairs);
+    const int pairs = b.mblocks * b.kblocks, sms = num_sms();
+    b.gx = pairs == 1 ? sms : (sms / pairs < 8 ? 8 : sms / pairs);
     return b;
 }
 
@@ -799,7 +798,8 @@ static void launch_gemm(const GemmArgs& g, int splits, cudaStream_t st) {
 
 static int elementwise_blocks(size_t total) {
     size_t b = (total + 255) / 256;
-    return (int)(b > 148 * 16 ? 148 * 16 : (b < 1 ? 1 : b));
+    const size_t cap = (size_t)num_sms() * 16;
+    return (int)(b > cap ? cap : (b < 1 ? 1 : b));
 }
 
 
@@ -849,19 +849,18 @@ static int opt_in_smem(K kernel, size_t bytes) {
 // picks the row-tile height R (32/16/8) and ring depth so the kernel's buffers fit the 227 KB of one SM
 static size_t wgrad_smem(int N, int K, int KP, int& R, int passes, int& stages, bool fused_dz = false, int min_R = 8) {
     // Largest tile height whose operand buffers and a >= 2-deep raw ring fit; as many ring stages as then fit.
-    const int p_chunks = (KP + 31) / 32;
     const size_t limit = 227 * 1024;
     static const int heights[] = {32, 24, 16, 8};
     auto fit = [&](int rows, int& st) -> size_t {
-        const size_t op = (size_t)(4 + p_chunks) * rows * 128 * (passes == 3 ? 2 : 1);
+        const size_t op = (size_t)(128 + KP) * 128 * (passes == 3 ? 2 : 1);      // transposed operands: one 128-byte chunk per row
         const size_t rawz = (((size_t)rows * N * 4 + 127) / 128 * 128) * (fused_dz ? 2 : 1), rawp = ((size_t)rows * K * 4 + 127) / 128 * 128;
         const size_t fixed = 1024 + 2 * op + 128 + 3 * 128 * 4;      // + barriers + the coefficient rows of the folded normalisation backward
         for (st = WG_MAX_STAGES; st >= 2; --st)
             if (fixed + st * (rawz + rawp) <= limit) return fixed + st * (rawz + rawp);
         return 0;
     };
-    // (measured on the box, PTRB200_WG_DEEP=1: 24-row tiles with a 4-deep ring are 2.5 % SLOWER on the headline step than
-    //  32-row tiles with 2 stages -- a quarter of the producer threads idle on a 24-row tile -- so depth is opt-in)
+    // (PTRB200_WG_DEEP=1 prefers ring depth over tile height: a 24-row tile leaves a quarter of the staging threads idle,
+    //  so by default the tallest tile that fits with 2 stages wins)
     static const bool deep = getenv("PTRB200_WG_DEEP") && getenv("PTRB200_WG_DEEP")[0] == '1';
     for (int pass = deep ? 0 : 1; pass < 2; ++pass)
         for (int h : heights) {
@@ -876,8 +875,8 @@ static size_t wgrad_smem(int N, int K, int KP, int& R, int passes, int& stages, 
 
 static bool rows_ws_fits(int K, int N, int passes) {
     const int NP = ((N + 15) / 16) * 16, nchunks = (K + 31) / 32;
-    const size_t ws_smem = 1024 + (size_t)nchunks * NP * 128 * (passes == 3 ? 2 : 1) + 65536 + (size_t)4 * NP * 8 + 128;
-    return ws_smem <= 227 * 1024 && N <= 256;
+    const size_t ws_smem = 1024 + (size_t)nchunks * NP * 128 * (passes == 3 ? 2 : 1) + 65536 + (size_t)RW_EPI_WARPS * NP * 8 + 128;
+    return ws_smem <= 227 * 1024 && N <= RW_MAX_N;
 }
 
 // stats_kind: 0 none, 1 one statistics group over the whole batch (BN), 2 per-query groups (BN2).
@@ -889,13 +888,13 @@ static int launch_rows_gemm(int mode, int passes, RowsGemmArgs& g, int ntiles, c
     int rc;
     const int nchunks = (g.K + 31) / 32;
     // ---- persistent warp-specialised kernel when the whole weight image fits beside the A ring ----
-    const size_t ws_smem = 1024 + (size_t)nchunks * g.NP * 128 * (passes == 3 ? 2 : 1) + 65536 + (size_t)4 * g.NP * 8 + 128;
+    const size_t ws_smem = 1024 + (size_t)nchunks * g.NP * 128 * (passes == 3 ? 2 : 1) + 65536 + (size_t)RW_EPI_WARPS * g.NP * 8 + 128;
     const bool seg_ok = !g.partials || g.seg_len == g.tile_rows || g.group_rows > 0;     // no sub-tile statistics segments
-    if (ws_smem <= 227 * 1024 && seg_ok && g.N <= 256) {
+    if (ws_smem <= 227 * 1024 && seg_ok && g.N <= RW_MAX_N) {
         RowsWsExtra x{};
         x.ntiles = ntiles; x.nchunks = nchunks;
         x.stats_mode = (!g.partials || stats_kind == 0) ? 0 : (stats_kind == 1 ? 1 : 2);
-        const int grid = ntiles < 148 ? ntiles : 148;
+        const int grid = ntiles < num_sms() ? ntiles : num_sms();
         if (S_out) *S_out = x.stats_mode == 1 ? grid : S_default;
 #define RW_CASE_K(M, P, A, KT, TAG)                                                                 \
         if (mode == M && passes == P && act_t == A && g.K == KT) {                                  \
@@ -932,11 +931,9 @@ static int launch_rows_gemm(int mode, int passes, RowsGemmArgs& g, int ntiles, c
         return PTRB200_ERR_INVALID;
     }
     if (S_out) *S_out = S_default;
-    // one-tile-per-CTA kernel; output columns are tiled (144 per CTA) when the layer is wider than one MMA tile likes
-    // (long contractions carry a second TMEM accumulator: 128-column tiles keep the pair inside 256 TMEM columns, so two CTAs
-    //  still share an SM; a layer of up to 144 outputs stays one tile -- it then takes all 512 columns)
-    const bool long_k = passes == 3 && nchunks > 5;
-    g.n_tile = g.N <= 144 ? g.N : (long_k ? 128 : 144);
+    // one-tile-per-CTA kernel; output columns are tiled (RG_MAX_N per CTA) when the layer is wider: the accumulators of
+    // a tile live in registers
+    g.n_tile = g.N <= RG_MAX_N ? g.N : RG_MAX_N;
     const int n_tiles = (g.N + g.n_tile - 1) / g.n_tile;
     const int NPt = ((g.n_tile + 15) / 16) * 16;
     const size_t operands = 32768 + (size_t)2 * NPt * 256, otile = (size_t)128 * g.n_tile * 4;      // A hi|lo + two weight-chunk stages
@@ -981,7 +978,7 @@ static void set_prologue(const ptrb200_ffnet* net, const Plan& p, int l, char* w
 // ------------------------------------------------------------------ per-query BN2 over a ragged batch (SURVEY 8f-2)
 // LTRBatchNorm2 (base/utils.py:227-282) normalises every query over its own documents.  With per-query offsets one CTA
 // owns one query (32 channel lanes x 8 row lanes), so moments, dY sums and the normalisation backward need no cross-CTA
-// reduction; the Linear contractions run on the same tcgen05 kernels in their plain (no fused prologue) form.
+// reduction; the Linear contractions run on the same tensor-core kernels in their plain (no fused prologue) form.
 __global__ void __launch_bounds__(256) bn2_ragged_moments_kernel(const float* __restrict__ Z, const int32_t* __restrict__ offsets,
                                                                   float* __restrict__ mean, float* __restrict__ rstd, int C) {
     __shared__ double sh1[8][33], sh2[8][33];
@@ -1309,7 +1306,7 @@ static int backward_tc(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grad
         dim3 sgrid(p.G, p.S_stat);
         // the backward statistics pass picks its own slicing: long slices amortise the per-CTA reduction
         int bS = p.S_stat, bslice = p.slice_rows;
-        // (measured: 128-row slices = 2048 CTAs beat longer slices; kept equal to the forward tiling)
+        // (128-row slices, equal to the forward tiling)
         if (lp.has_act || lp.has_norm) {
             float* dY = dbuf[flip]; flip ^= 1;
             launch_colstat<STAT_DY>(st, "colstat_dy", Z, dA, dY, nr, part, p.G, bS, p.gr, lp.d_out, bslice, r1);

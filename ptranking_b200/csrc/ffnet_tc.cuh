@@ -1,4 +1,4 @@
-// ffnet_tc.cuh -- tcgen05 layer kernels of the stacked feed-forward scorer.
+// ffnet_tc.cuh -- wgmma layer kernels of the stacked feed-forward scorer.
 //
 // Three kernels cover one Linear layer in both directions; post-activation tensors are never
 // written to HBM -- they are rebuilt from the previous layer's pre-activation Z in the operand
@@ -8,7 +8,7 @@
 //   rows_gemm<DGRAD>  dA[rows,K]   = dropmask( dZ_l * W )                           (Wt = W^T staged)
 //   wgrad             dW[N,K]      = sum_rows dZ_l[r,:]^T (x) drop(act(Z_{l-1}*scale+shift))[r,:]
 //
-// All contractions run as kind::tf32 tcgen05.mma with fp32 accumulation in TMEM; PASSES = 3 is the
+// All contractions run as tf32 wgmma with fp32 accumulation in registers; PASSES = 3 is the
 // error-compensated 3xTF32 split (fp32-equivalent, the default), PASSES = 1 plain TF32.
 #pragma once
 #include "common.cuh"
@@ -40,8 +40,8 @@ struct RowsGemmArgs {
     float* Out;            // [rows, N]
     double* partials;      // [slots, N, 2] column sum / sum of squares per statistics slot, or NULL
     int rows, K, N, NP;
-    int n_tile;            // one-tile-per-CTA kernel: output columns per CTA (gridDim.y tiles), multiple of 16; N when untiled
-    int tail_off;          // byte offset of the mbarrier / TMEM slot behind max(operand buffers, output tile)
+    int n_tile;            // one-tile-per-CTA kernel: output columns per CTA (gridDim.y tiles, <= RG_MAX_N); N when untiled
+    int tail_off;          // byte offset of the mbarriers behind max(operand buffers, output tile)
     // tile -> rows mapping
     int tile_rows;         // rows advanced per tile (<= 128)
     int seg_len;           // rows per statistics segment inside a tile
@@ -181,7 +181,8 @@ __global__ void pack_b_image_kernel(const float* __restrict__ src, int src_rows,
     }
 }
 
-constexpr int RG_THREADS = 256;
+constexpr int RG_THREADS = 256;         // two warpgroups, 64 rows of the 128-row tile each
+constexpr int RG_MAX_N = 128;           // output columns per CTA: the accumulators of a 64 x 128 warpgroup tile fill 64 registers
 
 template <int MODE, int PASSES, int ACT = -1>
 __global__ void __launch_bounds__(RG_THREADS) rows_gemm_tc_kernel(RowsGemmArgs g) {
@@ -199,12 +200,10 @@ __global__ void __launch_bounds__(RG_THREADS) rows_gemm_tc_kernel(RowsGemmArgs g
     unsigned char* b_buf = a_lo + 16384;
     const uint32_t b_stage = (uint32_t)NP * 128u * (PASSES == 3 ? 2u : 1u);
     unsigned char* tail = base + g.tail_off;
-    uint64_t* mbar = reinterpret_cast<uint64_t*>(tail);
-    uint64_t* bbar = mbar + 1;                        // [2]
-    uint32_t* slot = reinterpret_cast<uint32_t*>(mbar + 3);
+    uint64_t* bbar = reinterpret_cast<uint64_t*>(tail);   // [2] weight chunk landed
     float* otile = reinterpret_cast<float*>(base);    // epilogue staging [128][N], aliases the operand buffers
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, wg = tid >> 7;
     // ---- tile -> rows ------------------------------------------------------------
     int row0, nrows, slot0;
     {
@@ -220,23 +219,15 @@ __global__ void __launch_bounds__(RG_THREADS) rows_gemm_tc_kernel(RowsGemmArgs g
             slot0 = (row0 / g.seg_len);
         }
     }
-    // The tensor core accumulates with truncation: the error of a 3xTF32 contraction grows linearly with the number of
-    // accumulate steps (DESIGN.md 4).  Contractions longer than 5 chunks (K > 160: the 256- and 512-wide layers of the list
-    // scorer's head / tail nets) therefore keep the small a_lo*b_hi + a_hi*b_lo corrections in an accumulator of their own
-    // -- two thirds of the accumulate steps leave the main chain -- and stage A with the round-to-nearest split; the
-    // epilogue adds the two accumulators in round-to-nearest fp32.
+    // The error of a 3xTF32 contraction grows with the number of accumulate steps (DESIGN.md 4): the small
+    // a_lo*b_hi + a_hi*b_lo corrections accumulate apart from the main products (two thirds of the accumulate steps
+    // leave the main chain; the epilogue adds the two), and contractions longer than 5 chunks (K > 160: the 256- and
+    // 512-wide layers of the list scorer's head / tail nets) also stage A with the round-to-nearest split.
     const int K = g.K;
     const int nchunks = (K + 31) / 32;
     const bool long_k = PASSES == 3 && nchunks > 5;
-    const uint32_t need_cols = (uint32_t)(long_k ? 2 * NP : NP);
-    const uint32_t tmem_cols = need_cols <= 32 ? 32 : need_cols <= 64 ? 64 : need_cols <= 128 ? 128 : need_cols <= 256 ? 256 : 512;
-    if (tid == 0) { tc::mbar_init(mbar, 1); tc::mbar_init(bbar, 1); tc::mbar_init(bbar + 1, 1); tc::mbar_fence_init(); }
-    if (warp == 0) tc::tmem_alloc(slot, tmem_cols);
-    tc::fence_before_sync();
+    if (tid == 0) { tc::mbar_init(bbar, 1); tc::mbar_init(bbar + 1, 1); tc::mbar_fence_init(); }
     __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tmem = *slot;
-    const uint32_t idesc = tc::instr_desc(2, 128, NP);
     constexpr int A_UNITS = 128 * 8 / RG_THREADS;      // 4 units of 16 B per thread per chunk
     size_t coef_off[A_UNITS];                           // (statistics group of the thread's rows) * K
 #pragma unroll
@@ -247,7 +238,7 @@ __global__ void __launch_bounds__(RG_THREADS) rows_gemm_tc_kernel(RowsGemmArgs g
 
     // ---- global -> registers one chunk AHEAD: the loads of chunk c+1 fly while chunk c is staged, synchronised and
     // multiplied (a tile's chunks are strictly sequential and few CTAs share an SM at list-scorer row counts, so nothing
-    // else hides the HBM latency: measured 4 us per chunk without the prefetch) ----
+    // else hides the HBM latency) ----
     float4 nav[A_UNITS];
     auto load_chunk = [&](int c) {
 #pragma unroll
@@ -257,13 +248,18 @@ __global__ void __launch_bounds__(RG_THREADS) rows_gemm_tc_kernel(RowsGemmArgs g
         }
     };
     load_chunk(0);
+    tc::with_width(NP, [&](auto W) {
+    constexpr int NPc = decltype(W)::value;
+    float acc[NPc / 2], acc2[NPc / 2];
+#pragma unroll
+    for (int e = 0; e < NPc / 2; ++e) { acc[e] = 0.0f; acc2[e] = 0.0f; }
     for (int c = 0; c < nchunks; ++c) {
         const int k0 = c * 32;
         float4 av[A_UNITS];
 #pragma unroll
         for (int i = 0; i < A_UNITS; ++i) av[i] = nav[i];
         if (c + 1 < nchunks) load_chunk(c + 1);
-        if (c > 0) tc::mbar_wait(mbar, (c - 1) & 1);
+        if (c > 0) __syncthreads();                        // both warpgroups' MMAs of chunk c-1 are done with the A buffer and B stage
         // ---- B: one TMA bulk copy per operand image chunk (no SM instructions beyond the issue), one chunk ahead ----
         if (tid == 0) {
             auto fetch_b = [&](int cc) {
@@ -283,6 +279,15 @@ __global__ void __launch_bounds__(RG_THREADS) rows_gemm_tc_kernel(RowsGemmArgs g
             const int u = tid + i * RG_THREADS, r = u >> 3, j = u & 7, k = k0 + j * 4;
             float4 v = av[i];
             if (r < nrows && k < K) {
+                if (MODE == RG_DGRAD && g.P2) {                   // dZ = k1*dY + k3*Z + k0 (normalisation backward folded in)
+                    const size_t kc = (g.gr_cur < g.rows ? (size_t)((row0 + r) / g.gr_cur) * K : (size_t)0) + k;
+                    const float4 z = __ldg(reinterpret_cast<const float4*>(g.P2 + (size_t)(row0 + r) * K + k));
+                    const float4 a1 = __ldg(reinterpret_cast<const float4*>(g.kc1 + kc));
+                    const float4 a3 = __ldg(reinterpret_cast<const float4*>(g.kc3 + kc));
+                    const float4 a0 = __ldg(reinterpret_cast<const float4*>(g.kc0 + kc));
+                    v.x = fmaf(a1.x, v.x, fmaf(a3.x, z.x, a0.x)); v.y = fmaf(a1.y, v.y, fmaf(a3.y, z.y, a0.y));
+                    v.z = fmaf(a1.z, v.z, fmaf(a3.z, z.z, a0.z)); v.w = fmaf(a1.w, v.w, fmaf(a3.w, z.w, a0.w));
+                }
                 v = prologue4<ACT>(g, v, row0 + r, k, MODE == RG_FWD, coef_off[i]);
                 if (MODE == RG_FWD && g.a_out && blockIdx.y == 0) *reinterpret_cast<float4*>(g.a_out + (size_t)(row0 + r) * K + k) = v;
             } else v = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -290,83 +295,40 @@ __global__ void __launch_bounds__(RG_THREADS) rows_gemm_tc_kernel(RowsGemmArgs g
         }
         tc::fence_proxy_async();
         __syncthreads();
-        if (tid == 0) {
-            tc::mbar_wait(bbar + (c & 1), (c >> 1) & 1);      // weights chunk has landed
-            tc::fence_after_sync();
-            const int ksteps = min(4, (K - k0 + 7) / 8);
-            const uint32_t b_hi_s = tc::smem_u32(b_buf) + (uint32_t)(c & 1) * b_stage, b_lo_s = b_hi_s + (uint32_t)NP * 128u;
-            for (int s = 0; s < ksteps; ++s) {
-                const uint64_t ah = tc::smem_desc_sw128(tc::smem_u32(a_hi) + s * 32, 1024);
-                const uint64_t bh = tc::smem_desc_sw128(b_hi_s + s * 32, 1024);
-                const uint32_t acc = (c == 0 && s == 0) ? 0u : 1u;
-                if (PASSES == 3) {
-                    const uint64_t al = tc::smem_desc_sw128(tc::smem_u32(a_lo) + s * 32, 1024);
-                    const uint64_t bl = tc::smem_desc_sw128(b_lo_s + s * 32, 1024);
-                    if (long_k) {
-                        tc::mma_tf32(tmem + (uint32_t)NP, al, bh, idesc, acc);
-                        tc::mma_tf32(tmem + (uint32_t)NP, ah, bl, idesc, 1u);
-                        tc::mma_tf32(tmem, ah, bh, idesc, acc);
-                    } else {
-                        tc::mma_tf32(tmem, al, bh, idesc, acc);
-                        tc::mma_tf32(tmem, ah, bl, idesc, 1u);
-                        tc::mma_tf32(tmem, ah, bh, idesc, 1u);
-                    }
-                } else {
-                    tc::mma_tf32(tmem, ah, bh, idesc, acc);
-                }
+        tc::mbar_wait(bbar + (c & 1), (c >> 1) & 1);          // weights chunk has landed
+        const uint32_t a_s = tc::smem_u32(a_hi) + wg * 8192;
+        const uint32_t b_hi_s = tc::smem_u32(b_buf) + (uint32_t)(c & 1) * b_stage, b_lo_s = b_hi_s + (uint32_t)NP * 128u;
+        // four K-steps per chunk: the columns beyond K are staged as zeros, so a fixed chain keeps the wgmmas back to back
+        tc::wg_fence();
+#pragma unroll
+        for (int s = 0; s < 4; ++s) {
+            const uint64_t ah = tc::smem_desc_sw128(a_s + s * 32, 1024);
+            const uint64_t bh = tc::smem_desc_sw128(b_hi_s + s * 32, 1024);
+            if (PASSES == 3) {
+                const uint64_t al = tc::smem_desc_sw128(a_s + 16384 + s * 32, 1024);
+                const uint64_t bl = tc::smem_desc_sw128(b_lo_s + s * 32, 1024);
+                tc::mma_tf32<NPc>(acc2, al, bh, 1u);
+                tc::mma_tf32<NPc>(acc2, ah, bl, 1u);
             }
-            tc::mma_commit(mbar);
+            tc::mma_tf32<NPc>(acc, ah, bh, 1u);
         }
+        tc::wg_commit();
+        tc::wg_wait<0>();                                 // the same threads stage the next chunk: its registers are needed there
     }
-    tc::mbar_wait(mbar, (nchunks - 1) & 1);
-    tc::fence_after_sync();
+    __syncthreads();                                      // every MMA is done: the output tile may overwrite the operands
 
-    // ---- epilogue: TMEM -> registers -> (+bias | dropout mask) -> smem tile [128][N] ----
-    {
-        const int q = warp & 3, half = warp >> 2;                 // lane quarter, column half
-        const int r = q * 32 + lane;
-        const int cols_half = ((NP / 8 + 1) / 2) * 8;             // columns handled by half 0
-        const int c_begin = half == 0 ? 0 : cols_half, c_end = half == 0 ? min(cols_half, NP) : NP;
-        for (int c0 = c_begin; c0 < c_end; c0 += 8) {
-            float v[8];
-            tc::tmem_ld8(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-            if (long_k) {
-                float w[8];
-                tc::tmem_ld8(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(NP + c0), w);
+    // ---- epilogue: registers -> (+bias | dropout mask) -> smem tile [128][N] ----
 #pragma unroll
-                for (int e = 0; e < 8; ++e) v[e] += w[e];
-            }
-            if (c0 < N) {
-                if (MODE == RG_FWD) {
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) if (c0 + e < N) v[e] += __ldg(g.bias + n0 + c0 + e);
-                } else if (g.drop.thr) {
-                    if ((N_full & 3) == 0) {              // rows start on a draw boundary: 2 draws cover the 8 columns
-                        const uint64_t q = ((uint64_t)(row0 + r) * N_full + n0 + c0) >> 2;
-                        const uint64_t d0 = dropout_draw4(g.drop.key, q), d1 = dropout_draw4(g.drop.key, q + 1);
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            v[e] = ((uint32_t)(d0 >> (16 * e)) & 0xffffu) >= g.drop.thr ? v[e] * g.drop.scale : 0.0f;
-                            v[4 + e] = ((uint32_t)(d1 >> (16 * e)) & 0xffffu) >= g.drop.thr ? v[4 + e] * g.drop.scale : 0.0f;
-                        }
-                    } else {
-#pragma unroll
-                        for (int e = 0; e < 8; ++e)
-                            if (c0 + e < N) v[e] = dropout_keep(g.drop.key, (uint64_t)(row0 + r) * N_full + n0 + c0 + e, g.drop.thr) ? v[e] * g.drop.scale : 0.0f;
-                    }
-                }
-                float* dst = otile + (size_t)r * N + c0;
-                if (c0 + 8 <= N && (N & 3) == 0) {
-                    *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
-                    *reinterpret_cast<float4*>(dst + 4) = make_float4(v[4], v[5], v[6], v[7]);
-                } else {
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) if (c0 + e < N) dst[e] = v[e];
-                }
-            }
-        }
+    for (int e = 0; e < NPc / 2; ++e) {
+        const int r = wg * 64 + tc::acc_row(e), col = tc::acc_col(e);
+        if (col >= N) continue;
+        float v = PASSES == 3 ? acc[e] + acc2[e] : acc[e];
+        if (MODE == RG_FWD) v += __ldg(g.bias + n0 + col);
+        else if (g.drop.thr)
+            v = dropout_keep(g.drop.key, (uint64_t)(row0 + r) * N_full + n0 + col, g.drop.thr) ? v * g.drop.scale : 0.0f;
+        otile[(size_t)r * N + col] = v;
     }
-    tc::fence_before_sync();
+    });
     __syncthreads();
     // ---- tile -> global: contiguous when untiled, row segments of pitch N_full otherwise ----
     if (N == N_full) {
@@ -402,24 +364,26 @@ __global__ void __launch_bounds__(RG_THREADS) rows_gemm_tc_kernel(RowsGemmArgs g
             }
         }
     }
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tmem, tmem_cols);
 }
 
 // --------------------------------------------------------------------------------------------
 // rows_gemm, persistent warp-specialised variant (used whenever the whole weight image fits next to the
 // A ring in shared memory, i.e. for every layer of the pointwise scorer).
 //
-//   warps 0-7   epilogue : TMEM -> registers -> (+bias | dropout mask) -> global rows, BN column sums
-//   warp  8     control  : one-time TMA bulk load of the resident W image; per K-chunk tcgen05.mma issue
-//   warps 9-24  producers: global -> registers (prefetched one chunk ahead) -> prologue -> hi/lo split ->
+//   warps 0-7   consumers: two warpgroups, 64 rows of the tile each; one-time TMA bulk load of the resident
+//                          W image, per K-chunk wgmma issue, epilogue registers -> (+bias | dropout mask) ->
+//                          global rows, BN column sums
+//   warps 8-15  producers: global -> registers (prefetched one chunk ahead) -> prologue -> hi/lo split ->
 //                          swizzled A stage (ring of 2)
-// TMEM holds two accumulators so the epilogue of tile t overlaps the MMAs of tile t+1; producers, control
-// and epilogue only meet through mbarriers (aready/afree per A stage, accfull/accfree per accumulator).
+// Producers and consumers only meet through mbarriers (aready/afree per A stage): the producers stage tile t+1
+// while the consumers multiply and write out tile t.  512 threads leave 128 registers per thread, room for a
+// 64 x 128 accumulator per consumer thread and the producers' four prefetched units.
 // --------------------------------------------------------------------------------------------
-constexpr int RW_EPI_WARPS = 8, RW_PROD_WARPS = 16;      // epilogue: 2 warps per TMEM lane quarter (column halves)
-constexpr int RW_THREADS = (RW_EPI_WARPS + 1 + RW_PROD_WARPS) * 32;
+constexpr int RW_EPI_WARPS = 8, RW_PROD_WARPS = 8;
+constexpr int RW_THREADS = (RW_EPI_WARPS + RW_PROD_WARPS) * 32;
 constexpr int RW_PRODUCERS = RW_PROD_WARPS * 32;
+constexpr int RW_PU = 128 * 8 / RW_PRODUCERS;            // 16-byte A units per producer thread per chunk
+constexpr int RW_MAX_N = 128;
 
 struct RowsWsExtra {
     int ntiles;
@@ -438,28 +402,6 @@ static __device__ __forceinline__ void rw_tile(const RowsGemmArgs& g, int t, int
     }
 }
 
-// sum of v[i] over the 32 lanes for 8 values per lane: 9 shuffles; every lane returns the total of column
-// ((lane>>4)&1)*4 + ((lane>>3)&1)*2 + ((lane>>2)&1)
-static __device__ __forceinline__ float warp_colsum8(const float (&v)[8], int lane) {
-    float a[4], b[2];
-    const bool h16 = lane & 16, h8 = lane & 8, h4 = lane & 4;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const float mine = h16 ? v[4 + i] : v[i], other = h16 ? v[i] : v[4 + i];
-        a[i] = mine + __shfl_xor_sync(0xffffffffu, other, 16);
-    }
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-        const float mine = h8 ? a[2 + i] : a[i], other = h8 ? a[i] : a[2 + i];
-        b[i] = mine + __shfl_xor_sync(0xffffffffu, other, 8);
-    }
-    const float mine = h4 ? b[1] : b[0], other = h4 ? b[0] : b[1];
-    float c = mine + __shfl_xor_sync(0xffffffffu, other, 4);
-    c += __shfl_xor_sync(0xffffffffu, c, 1);
-    c += __shfl_xor_sync(0xffffffffu, c, 2);
-    return c;
-}
-
 // ACT: the prologue activation as a compile-time constant (PTRB200_AF_*), or -1 to read g.act at run time
 // KT:  the contraction width as a compile-time constant (0 = read g.K at run time).  The producers spend more instructions
 //      on row / chunk address arithmetic, bounds predicates and the prefetch bookkeeping than on the prologue itself; with
@@ -474,105 +416,49 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
     unsigned char* w_hi = base;                                   // [nchunks][NP][128 B]
     unsigned char* w_lo = w_hi + (size_t)nchunks * wchunk;
     unsigned char* a_ring = w_lo + (PASSES == 3 ? (size_t)nchunks * wchunk : 0);   // [2][hi 16 KB | lo 16 KB]
-    float* stat_sm = reinterpret_cast<float*>(a_ring + 2 * 32768);                 // [4 lane quarters][NP][2]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(stat_sm + 4 * NP * 2);
+    float* stat_sm = reinterpret_cast<float*>(a_ring + 2 * 32768);                 // [8 consumer warps][NP][2]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(stat_sm + RW_EPI_WARPS * NP * 2);
     uint64_t* wfull = bars;            // W image landed
     uint64_t* aready = bars + 1;       // [2] A stage staged            (one arrive per producer warp)
-    uint64_t* afree = bars + 3;        // [2] MMAs done with the stage  (tcgen05.commit)
-    uint64_t* accfull = bars + 5;      // [2] accumulator complete      (tcgen05.commit)
-    uint64_t* accfree = bars + 7;      // [2] accumulator drained       (one arrive per epilogue warp)
-    uint32_t* slot = reinterpret_cast<uint32_t*>(bars + 9);
+    uint64_t* afree = bars + 3;        // [2] MMAs done with the stage  (one arrive per consumer warp)
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const uint32_t acc_cols = NP <= 32 ? 32 : NP <= 64 ? 64 : NP <= 128 ? 128 : 256;   // one accumulator
-    const uint32_t tmem_cols = acc_cols * 2;
     if (tid == 0) {
         tc::mbar_init(wfull, 1);
-        for (int i = 0; i < 2; ++i) { tc::mbar_init(aready + i, RW_PROD_WARPS); tc::mbar_init(afree + i, 1); tc::mbar_init(accfull + i, 1); tc::mbar_init(accfree + i, RW_EPI_WARPS); }
+        for (int i = 0; i < 2; ++i) { tc::mbar_init(aready + i, RW_PROD_WARPS); tc::mbar_init(afree + i, RW_EPI_WARPS); }
         tc::mbar_fence_init();
     }
-    if (warp == 0) tc::tmem_alloc(slot, tmem_cols);
-    tc::fence_before_sync();
     __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tmem = *slot;
     const int my_tiles = blockIdx.x < x.ntiles ? (x.ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
 
-    if (warp == RW_EPI_WARPS) {
-        // ================================ control warp ================================
-        // the whole warp runs the loop (warp-uniform descriptors); one elected lane issues TMA / MMA / commit
-        if (my_tiles > 0) {
-            const uint32_t idesc = tc::instr_desc(2, 128, NP);
-            const bool leader = tc::elect_one();
-            if (leader) {
-                tc::mbar_expect_tx(wfull, (uint32_t)(nchunks * wchunk * (PASSES == 3 ? 2 : 1)));
-                for (int c = 0; c < nchunks; ++c) {
-                    tc::bulk_g2s(w_hi + (size_t)c * wchunk, g.b_img_hi + (size_t)c * wchunk, wchunk, wfull);
-                    if (PASSES == 3) tc::bulk_g2s(w_lo + (size_t)c * wchunk, g.b_img_lo + (size_t)c * wchunk, wchunk, wfull);
-                }
-            }
-            tc::mbar_wait(wfull, 0);
-            const uint32_t a_base = tc::smem_u32(a_ring), wh_base = tc::smem_u32(w_hi), wl_base = tc::smem_u32(w_lo);
-            int q = 0;
-            for (int it = 0; it < my_tiles; ++it) {
-                const int b = it & 1;
-                if (it >= 2) tc::mbar_wait(accfree + b, ((it - 2) >> 1) & 1);
-                tc::fence_after_sync();
-                const uint32_t dacc = tmem + (uint32_t)b * acc_cols;
-    #pragma unroll (KT ? 8 : 1)
-            for (int c = 0; c < nchunks; ++c, ++q) {
-                    const int s = q & 1;
-                    tc::mbar_wait(aready + s, (q >> 1) & 1);
-                    tc::fence_after_sync();
-                    const uint32_t a_addr = a_base + s * 32768;
-                    uint64_t ah = tc::smem_desc_sw128(a_addr, 1024), al = tc::smem_desc_sw128(a_addr + 16384, 1024);
-                    uint64_t bh = tc::smem_desc_sw128(wh_base + c * wchunk, 1024), bl = tc::smem_desc_sw128(wl_base + c * wchunk, 1024);
-                    const int ksteps = min(4, (K - c * 32 + 7) / 8);
-                    if (leader) {
-                        for (int st = 0; st < ksteps; ++st) {
-                            const uint32_t acc = (c == 0 && st == 0) ? 0u : 1u;
-                            if (PASSES == 3) {
-                                tc::mma_tf32(dacc, al, bh, idesc, acc);
-                                tc::mma_tf32(dacc, ah, bl, idesc, 1u);
-                                tc::mma_tf32(dacc, ah, bh, idesc, 1u);
-                            } else {
-                                tc::mma_tf32(dacc, ah, bh, idesc, acc);
-                            }
-                            ah += 2; al += 2; bh += 2; bl += 2;          // +32 B along K inside the swizzle atom
-                        }
-                        tc::mma_commit(afree + s);
-                        if (c == nchunks - 1) tc::mma_commit(accfull + b);
-                    }
-                    __syncwarp();
-                }
-            }
-        }
-    } else if (warp > RW_EPI_WARPS) {
+    if (warp >= RW_EPI_WARPS) {
         if constexpr (MODE == RG_DGRAD) {
-        // (the data-gradient instantiation keeps the round-1 producer loop verbatim: its fused dZ = k1*dY + k3*Z + k0 staging sits
-        //  at the 72-register cap, and the restructured loop below spills there -- measured 0.48 -> 0.63 ms per step)
+        // (the data-gradient instantiation keeps the simpler producer loop: its fused dZ = k1*dY + k3*Z + k0 staging carries
+        //  more live state, and the restructured loop below would add to it)
             // ================================ producer warps ================================
-            const int ptid = tid - (RW_EPI_WARPS + 1) * 32;
+            const int ptid = tid - RW_EPI_WARPS * 32;
             const int j4 = (ptid & 7) * 4;                              // first column of this thread's 16-byte unit inside a chunk
-            const int r_[2] = {ptid >> 3, (ptid >> 3) + 64};
-            const uint32_t sw_[2] = {tc::swz_offset(r_[0], ptid & 7), tc::swz_offset(r_[1], ptid & 7)};
+            int r_[RW_PU];
+            uint32_t sw_[RW_PU];
+    #pragma unroll
+            for (int i = 0; i < RW_PU; ++i) { r_[i] = (ptid >> 3) + i * (RW_PRODUCERS / 8); sw_[i] = tc::swz_offset(r_[i], ptid & 7); }
             const int total_q = my_tiles * nchunks;
             const bool has_coef = g.scale != nullptr;
             const bool per_group = has_coef && g.gr_prev < g.rows;
             const bool fused_dz = MODE == RG_DGRAD && g.P2 != nullptr;
-            float4 pre[2], pre2[2];
-            size_t soff[2];                                             // row * K + j4 for the tile being fetched
-            bool ok[2];
+            float4 pre[RW_PU], pre2[RW_PU];
+            size_t soff[RW_PU];                                         // row * K + j4 for the tile being fetched
+            bool ok[RW_PU];
             auto point = [&](int it) {                                  // set soff/ok for tile `it`
                 int r0, nr;
                 rw_tile(g, blockIdx.x + it * gridDim.x, r0, nr);
     #pragma unroll
-                for (int i = 0; i < 2; ++i) { ok[i] = r_[i] < nr; soff[i] = (size_t)(r0 + min(r_[i], nr - 1)) * K + j4; }
+                for (int i = 0; i < RW_PU; ++i) { ok[i] = r_[i] < nr; soff[i] = (size_t)(r0 + min(r_[i], nr - 1)) * K + j4; }
             };
             auto fetch = [&](int c) {
                 const bool kv = c * 32 + j4 < K;
     #pragma unroll
-                for (int i = 0; i < 2; ++i) {
+                for (int i = 0; i < RW_PU; ++i) {
                     pre[i] = (ok[i] && kv) ? __ldg(reinterpret_cast<const float4*>(g.P + soff[i] + c * 32)) : make_float4(0.f, 0.f, 0.f, 0.f);
                     if (MODE == RG_DGRAD) pre2[i] = (fused_dz && ok[i] && kv) ? __ldg(reinterpret_cast<const float4*>(g.P2 + soff[i] + c * 32)) : make_float4(0.f, 0.f, 0.f, 0.f);
                 }
@@ -583,14 +469,14 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
                 int row0, nrows;
                 rw_tile(g, blockIdx.x + it * gridDim.x, row0, nrows);
                 // per-tile invariants of this thread's two rows
-                bool live[2];
-                float* aout[2];
-                const float* sc[2];
-                const float* sh[2];
-                size_t kco[2];
-                uint64_t dq[2];
+                bool live[RW_PU];
+                float* aout[RW_PU];
+                const float* sc[RW_PU];
+                const float* sh[RW_PU];
+                size_t kco[RW_PU];
+                uint64_t dq[RW_PU];
     #pragma unroll
-                for (int i = 0; i < 2; ++i) {
+                for (int i = 0; i < RW_PU; ++i) {
                     live[i] = r_[i] < nrows;
                     const size_t e0 = (size_t)(row0 + min(r_[i], nrows - 1)) * K + j4;
                     aout[i] = (MODE == RG_FWD && g.a_out) ? g.a_out + e0 : nullptr;
@@ -603,8 +489,9 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
     #pragma unroll 1
             for (int c = 0; c < nchunks; ++c, ++q) {
                     const int s = q & 1;
-                    const float4 cur[2] = {pre[0], pre[1]};
-                    const float4 cur2[2] = {pre2[0], pre2[1]};
+                    float4 cur[RW_PU], cur2[RW_PU];
+    #pragma unroll
+                    for (int i = 0; i < RW_PU; ++i) { cur[i] = pre[i]; cur2[i] = pre2[i]; }
                     if (q + 1 < total_q) {                              // prefetch the next chunk (possibly of the next tile)
                         if (c + 1 < nchunks) fetch(c + 1); else { point(it + 1); fetch(0); }
                     }
@@ -612,7 +499,7 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
                     unsigned char* a_hi = a_ring + s * 32768;
                     const bool kv = c * 32 + j4 < K;
     #pragma unroll
-                    for (int i = 0; i < 2; ++i) {
+                    for (int i = 0; i < RW_PU; ++i) {
                         float4 v = cur[i];
                         if (live[i] && kv) {
                             if (MODE == RG_DGRAD && fused_dz) {           // dZ = k1*dY + k3*Z + k0
@@ -650,10 +537,12 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
             }
         } else {
             // ================================ producer warps ================================
-            const int ptid = tid - (RW_EPI_WARPS + 1) * 32;
+            const int ptid = tid - RW_EPI_WARPS * 32;
             const int j4 = (ptid & 7) * 4;                              // first column of this thread's 16-byte unit inside a chunk
-            const int r_[2] = {ptid >> 3, (ptid >> 3) + 64};
-            const uint32_t sw_[2] = {tc::swz_offset(r_[0], ptid & 7), tc::swz_offset(r_[1], ptid & 7)};
+            int r_[RW_PU];
+            uint32_t sw_[RW_PU];
+    #pragma unroll
+            for (int i = 0; i < RW_PU; ++i) { r_[i] = (ptid >> 3) + i * (RW_PRODUCERS / 8); sw_[i] = tc::swz_offset(r_[i], ptid & 7); }
             const int total_q = my_tiles * nchunks;
             const bool has_coef = g.scale != nullptr;
             const bool per_group = has_coef && g.gr_prev < g.rows;
@@ -661,24 +550,25 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
             // A width that is not a multiple of 32 leaves the LAST K-chunk mostly empty (K = 100: 4 of its 32 columns).  With
             // the regular mapping (8 units per row) 7 of every 8 lanes would run the whole prologue on nothing, so that chunk
             // uses a unit-major mapping instead: unit jB = (ptid >> 7) + 4 i of row rB = ptid & 127 -- whole warps share jB
-            // and only those below `zfill` (the units the chunk's MMA K-steps read) do any work; units in [vlast, zfill) are
-            // written as zeros.  22 % of the staging work of a 100-wide layer disappears.
+            // and only those below `vlast` run the prologue; units in [vlast, 8) are written as zeros (the MMAs read all four
+            // K-steps of every chunk).
             const int lastc = nchunks - 1;
             const int vlast = (K - lastc * 32 + 3) >> 2;                // 16-byte units of the last chunk that hold data (1..8)
-            // (forward only: in the dgrad instantiation the extra live state pushes the producers past 72 registers -- measured
-            //  +30 % on that kernel -- so it keeps the regular mapping)
+            // (forward only: the dgrad instantiation keeps the regular mapping, its fused staging already carries more live state)
             const bool partial = MODE == RG_FWD && vlast < 8 && !g.no_partial;
-            const int zfill = 2 * min(4, (K - lastc * 32 + 7) / 8);     // units the last chunk's MMAs read
+            const int zfill = 8;                                        // units the last chunk's MMAs read
             const int rB = ptid & 127;
-            const int jB_[2] = {ptid >> 7, (ptid >> 7) + 4};
-            float4 pre[2], pre2[2];
-            size_t soff[2], soffB[2];                                   // element offset of the thread's units in the tile being fetched
-            bool ok[2], okB[2];
+            int jB_[RW_PU];
+    #pragma unroll
+            for (int i = 0; i < RW_PU; ++i) jB_[i] = (ptid >> 7) + i * (RW_PRODUCERS / 128);
+            float4 pre[RW_PU], pre2[RW_PU];
+            size_t soff[RW_PU], soffB[RW_PU];                           // element offset of the thread's units in the tile being fetched
+            bool ok[RW_PU], okB[RW_PU];
             auto point = [&](int it) {                                  // set soff/ok for tile `it`
                 int r0, nr;
                 rw_tile(g, blockIdx.x + it * gridDim.x, r0, nr);
     #pragma unroll
-                for (int i = 0; i < 2; ++i) {
+                for (int i = 0; i < RW_PU; ++i) {
                     ok[i] = r_[i] < nr; soff[i] = (size_t)(r0 + min(r_[i], nr - 1)) * K + j4;
                     okB[i] = rB < nr && jB_[i] < vlast; soffB[i] = (size_t)(r0 + min(rB, nr - 1)) * K + lastc * 32 + min(jB_[i], vlast - 1) * 4;
                 }
@@ -686,7 +576,7 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
             auto fetch = [&](int c) {
                 if (partial && c == lastc) {
     #pragma unroll
-                    for (int i = 0; i < 2; ++i) {
+                    for (int i = 0; i < RW_PU; ++i) {
                         pre[i] = okB[i] ? __ldg(reinterpret_cast<const float4*>(g.P + soffB[i])) : make_float4(0.f, 0.f, 0.f, 0.f);
                         if (MODE == RG_DGRAD) pre2[i] = (fused_dz && okB[i]) ? __ldg(reinterpret_cast<const float4*>(g.P2 + soffB[i])) : make_float4(0.f, 0.f, 0.f, 0.f);
                     }
@@ -694,7 +584,7 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
                 }
                 const bool kv = c * 32 + j4 < K;
     #pragma unroll
-                for (int i = 0; i < 2; ++i) {
+                for (int i = 0; i < RW_PU; ++i) {
                     pre[i] = (ok[i] && kv) ? __ldg(reinterpret_cast<const float4*>(g.P + soff[i] + c * 32)) : make_float4(0.f, 0.f, 0.f, 0.f);
                     if (MODE == RG_DGRAD) pre2[i] = (fused_dz && ok[i] && kv) ? __ldg(reinterpret_cast<const float4*>(g.P2 + soff[i] + c * 32)) : make_float4(0.f, 0.f, 0.f, 0.f);
                 }
@@ -733,14 +623,14 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
                 int row0, nrows;
                 rw_tile(g, blockIdx.x + it * gridDim.x, row0, nrows);
                 // per-tile invariants of this thread's two rows
-                bool live[2];
-                float* aout[2];
-                const float* sc[2];
-                const float* sh[2];
-                size_t kco[2];
-                uint64_t dq[2];
+                bool live[RW_PU];
+                float* aout[RW_PU];
+                const float* sc[RW_PU];
+                const float* sh[RW_PU];
+                size_t kco[RW_PU];
+                uint64_t dq[RW_PU];
     #pragma unroll
-                for (int i = 0; i < 2; ++i) {
+                for (int i = 0; i < RW_PU; ++i) {
                     live[i] = r_[i] < nrows;
                     const size_t e0 = (size_t)(row0 + min(r_[i], nrows - 1)) * K + j4;
                     aout[i] = (MODE == RG_FWD && g.a_out) ? g.a_out + e0 : nullptr;
@@ -753,8 +643,9 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
     #pragma unroll (KT ? 8 : 1)
             for (int c = 0; c < nchunks; ++c, ++q) {
                     const int s = q & 1;
-                    const float4 cur[2] = {pre[0], pre[1]};
-                    const float4 cur2[2] = {pre2[0], pre2[1]};
+                    float4 cur[RW_PU], cur2[RW_PU];
+    #pragma unroll
+                    for (int i = 0; i < RW_PU; ++i) { cur[i] = pre[i]; cur2[i] = pre2[i]; }
                     if (q + 1 < total_q) {                              // prefetch the next chunk (possibly of the next tile)
                         if (c + 1 < nchunks) fetch(c + 1); else { point(it + 1); fetch(0); }
                     }
@@ -763,7 +654,7 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
                     if (partial && c == lastc) {
                         // unit-major mapping of the short last chunk: warps whose unit lies beyond `zfill` have nothing to do
     #pragma unroll
-                        for (int i = 0; i < 2; ++i) {
+                        for (int i = 0; i < RW_PU; ++i) {
                             const int jB = jB_[i];
                             if (jB < zfill) {
                                 float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -781,7 +672,7 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
                     } else {
                         const bool kv = c * 32 + j4 < K;
     #pragma unroll
-                        for (int i = 0; i < 2; ++i) {
+                        for (int i = 0; i < RW_PU; ++i) {
                             float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
                             if (live[i] && kv)
                                 v = xform(cur[i], cur2[i], has_coef ? sc[i] + c * 32 : nullptr, has_coef ? sh[i] + c * 32 : nullptr,
@@ -795,87 +686,115 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
                 }
             }
         }
-    } else {
-        // ================================ epilogue warps (0..7) ================================
-        // warp w reads TMEM lanes [32*(w&3), +32) (hardware restriction: lane quarter = warp id mod 4) and the
-        // column half (w>>2) of the accumulator, 16 columns per tcgen05.ld.
-        const int quarter = warp & 3, half = warp >> 2;
-        const int r = quarter * 32 + lane;                    // TMEM lane = row inside the tile
-        const int ch_cols = ((NP / 16 + 1) / 2) * 16;         // columns of half 0 (multiple of 16)
-        const int c_begin = half == 0 ? 0 : ch_cols, c_end = half == 0 ? min(ch_cols, NP) : NP;
+    } else if (my_tiles > 0) {
+        // ================================ consumer warps (0..7) ================================
+        // warpgroup wg multiplies rows [64 wg, +64) of every tile; the accumulator of the tile stays in registers
+        const int wg = warp >> 2;
+        if (tid == 0) {
+            tc::mbar_expect_tx(wfull, (uint32_t)(nchunks * wchunk * (PASSES == 3 ? 2 : 1)));
+            for (int c = 0; c < nchunks; ++c) {
+                tc::bulk_g2s(w_hi + (size_t)c * wchunk, g.b_img_hi + (size_t)c * wchunk, wchunk, wfull);
+                if (PASSES == 3) tc::bulk_g2s(w_lo + (size_t)c * wchunk, g.b_img_lo + (size_t)c * wchunk, wchunk, wfull);
+            }
+        }
+        tc::mbar_wait(wfull, 0);
+        const uint32_t a_base = tc::smem_u32(a_ring) + wg * 8192, wh_base = tc::smem_u32(w_hi), wl_base = tc::smem_u32(w_lo);
         double acc1 = 0.0, acc2 = 0.0;                        // per-CTA column sums for column `tid` (tid < 256)
+        tc::with_width(NP, [&](auto W) {
+        constexpr int NPc = decltype(W)::value;
+        int q = 0;
         for (int it = 0; it < my_tiles; ++it) {
-            const int b = it & 1, t = blockIdx.x + it * gridDim.x;
+            const int t = blockIdx.x + it * gridDim.x;
             int row0, nrows;
             rw_tile(g, t, row0, nrows);
-            const bool live = r < nrows;
-            tc::mbar_wait_relaxed(accfull + b, (it >> 1) & 1);
-            tc::fence_after_sync();
-            const uint32_t tbase = tmem + ((uint32_t)(quarter * 32) << 16) + (uint32_t)b * acc_cols;
-            float* orow = g.Out + (size_t)(row0 + min(r, nrows - 1)) * N;
-            for (int c0 = c_begin; c0 < c_end; c0 += 16) {
-                float v[16];
-                tc::tmem_ld16(tbase + (uint32_t)c0, v);
-                if (c0 >= N) continue;
+            float acc[NPc / 2];
 #pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-                    const int cc = c0 + hh * 8;
-                    float* w = v + hh * 8;
-                    if (cc >= N) break;
-                    if (MODE == RG_FWD) {
-                        if (cc + 8 <= N && (N & 3) == 0) {
-                            const float4 b0 = __ldg(reinterpret_cast<const float4*>(g.bias + cc)), b1 = __ldg(reinterpret_cast<const float4*>(g.bias + cc + 4));
-                            w[0] += b0.x; w[1] += b0.y; w[2] += b0.z; w[3] += b0.w; w[4] += b1.x; w[5] += b1.y; w[6] += b1.z; w[7] += b1.w;
-                        } else {
+            for (int e = 0; e < NPc / 2; ++e) acc[e] = 0.0f;
+    #pragma unroll (KT ? 8 : 1)
+            for (int c = 0; c < nchunks; ++c, ++q) {
+                const int s = q & 1;
+                tc::mbar_wait(aready + s, (q >> 1) & 1);
+                const uint32_t a_addr = a_base + s * 32768;
+                const uint64_t ah = tc::smem_desc_sw128(a_addr, 1024), al = tc::smem_desc_sw128(a_addr + 16384, 1024);
+                const uint64_t bh = tc::smem_desc_sw128(wh_base + c * wchunk, 1024), bl = tc::smem_desc_sw128(wl_base + c * wchunk, 1024);
+                // four K-steps per chunk (+32 B along K inside the swizzle atom each; columns beyond K are staged as zeros)
+                tc::wg_fence();
 #pragma unroll
-                            for (int e = 0; e < 8; ++e) w[e] = (cc + e < N) ? w[e] + __ldg(g.bias + cc + e) : 0.0f;
-                        }
-                    } else if (g.drop.thr) {
-                        if ((N & 3) == 0) {
-                            const uint64_t qd = ((uint64_t)(row0 + r) * N + cc) >> 2;
-                            const uint64_t d0 = dropout_draw4(g.drop.key, qd), d1 = dropout_draw4(g.drop.key, qd + 1);
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                w[e] = ((uint32_t)(d0 >> (16 * e)) & 0xffffu) >= g.drop.thr ? w[e] * g.drop.scale : 0.0f;
-                                w[4 + e] = ((uint32_t)(d1 >> (16 * e)) & 0xffffu) >= g.drop.thr ? w[4 + e] * g.drop.scale : 0.0f;
-                            }
-                        } else {
-#pragma unroll
-                            for (int e = 0; e < 8; ++e)
-                                if (cc + e < N) w[e] = dropout_keep(g.drop.key, (uint64_t)(row0 + r) * N + cc + e, g.drop.thr) ? w[e] * g.drop.scale : 0.0f;
-                        }
+                for (int st = 0; st < 4; ++st) {
+                    if (PASSES == 3) {
+                        tc::mma_tf32<NPc>(acc, al + 2 * st, bh + 2 * st, 1u);
+                        tc::mma_tf32<NPc>(acc, ah + 2 * st, bl + 2 * st, 1u);
                     }
-                    if (live) {
-                        if (cc + 8 <= N && (N & 3) == 0) {
-                            *reinterpret_cast<float4*>(orow + cc) = make_float4(w[0], w[1], w[2], w[3]);
-                            *reinterpret_cast<float4*>(orow + cc + 4) = make_float4(w[4], w[5], w[6], w[7]);
-                        } else {
+                    tc::mma_tf32<NPc>(acc, ah + 2 * st, bh + 2 * st, 1u);
+                }
+                tc::wg_commit();
+                // the MMAs of the previous chunk have completed: release its A stage
+                tc::wg_wait<1>();
+                if (c > 0) { __syncwarp(); if (lane == 0) tc::mbar_arrive(afree + (s ^ 1)); }
+            }
+            tc::wg_wait<0>();
+            __syncwarp();
+            if (lane == 0) tc::mbar_arrive(afree + ((q - 1) & 1));
+            // ---- epilogue: registers -> (+bias | dropout mask) -> global rows, per-warp column sums ----
+            bool live[2];
+            float* orow[2];
 #pragma unroll
-                            for (int e = 0; e < 8; ++e) if (cc + e < N) orow[cc + e] = w[e];
-                        }
+            for (int h = 0; h < 2; ++h) {
+                const int r = wg * 64 + tc::acc_row(2 * h);
+                live[h] = r < nrows;
+                orow[h] = g.Out + (size_t)(row0 + min(r, nrows - 1)) * N;
+            }
+#pragma unroll
+            for (int e = 0; e < NPc / 2; ++e) {
+                const int col = tc::acc_col(e);
+                if (col >= N) { acc[e] = 0.0f; continue; }
+                if (MODE == RG_FWD) acc[e] += __ldg(g.bias + col);
+                else if (g.drop.thr) {
+                    const int r = wg * 64 + tc::acc_row(e);
+                    acc[e] = dropout_keep(g.drop.key, (uint64_t)(row0 + r) * N + col, g.drop.thr) ? acc[e] * g.drop.scale : 0.0f;
+                }
+            }
+            // a thread holds two adjacent columns of two rows per 8-column group: 8-byte stores when N is even
+#pragma unroll
+            for (int e = 0; e < NPc / 2; e += 2) {
+                const int col = tc::acc_col(e), h = (e >> 1) & 1;
+                if (!live[h] || col >= N) continue;
+                if ((N & 1) == 0) *reinterpret_cast<float2*>(orow[h] + col) = make_float2(acc[e], acc[e + 1]);
+                else { orow[h][col] = acc[e]; if (col + 1 < N) orow[h][col + 1] = acc[e + 1]; }
+            }
+            if (MODE == RG_FWD && x.stats_mode) {
+#pragma unroll
+                for (int j = 0; j < NPc / 16; ++j) {
+                    const float* w = acc + 8 * j;
+                    // column sums over the warp's 16 rows: lanes with equal lane % 4 hold the same columns
+                    float s1[4], s2[4];
+#pragma unroll
+                    for (int p = 0; p < 4; ++p) {              // p = 2 * (e >> 2) + (e & 1): the four columns of this lane
+                        const int e0 = (p >> 1) * 4 + (p & 1), e1 = e0 + 2;
+                        const float v0 = live[0] ? w[e0] : 0.0f, v1 = live[1] ? w[e1] : 0.0f;
+                        s1[p] = v0 + v1; s2[p] = v0 * v0 + v1 * v1;
                     }
-                    if (MODE == RG_FWD && x.stats_mode) {
-                        float w1[8], w2[8];
 #pragma unroll
-                        for (int e = 0; e < 8; ++e) { w1[e] = live ? w[e] : 0.0f; w2[e] = w1[e] * w1[e]; }
-                        const float s1 = warp_colsum8(w1, lane), s2 = warp_colsum8(w2, lane);
-                        if ((lane & 3) == 0) {
-                            const int col = cc + ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);
-                            stat_sm[(quarter * NP + col) * 2] = s1;
-                            stat_sm[(quarter * NP + col) * 2 + 1] = s2;
+                    for (int p = 0; p < 4; ++p)
+#pragma unroll
+                        for (int o = 4; o < 32; o <<= 1) {
+                            s1[p] += __shfl_xor_sync(0xffffffffu, s1[p], o);
+                            s2[p] += __shfl_xor_sync(0xffffffffu, s2[p], o);
+                        }
+                    if (lane < 4) {
+#pragma unroll
+                        for (int p = 0; p < 4; ++p) {
+                            const int col = j * 16 + (p >> 1) * 8 + 2 * lane + (p & 1);
+                            stat_sm[(warp * NP + col) * 2] = s1[p];
+                            stat_sm[(warp * NP + col) * 2 + 1] = s2[p];
                         }
                     }
                 }
-            }
-            tc::fence_before_sync();
-            __syncwarp();
-            if (lane == 0) tc::mbar_arrive(accfree + b);
-            if (MODE == RG_FWD && x.stats_mode) {
                 asm volatile("bar.sync 2, 256;" ::: "memory");               // the 8 warps' column sums are in smem
                 if (tid < N) {
                     double s1 = 0.0, s2 = 0.0;
 #pragma unroll
-                    for (int w = 0; w < 4; ++w) { s1 += (double)stat_sm[(w * NP + tid) * 2]; s2 += (double)stat_sm[(w * NP + tid) * 2 + 1]; }
+                    for (int w = 0; w < RW_EPI_WARPS; ++w) { s1 += (double)stat_sm[(w * NP + tid) * 2]; s2 += (double)stat_sm[(w * NP + tid) * 2 + 1]; }
                     if (x.stats_mode == 2) {
                         double* p = g.partials + ((size_t)t * N + tid) * 2;
                         p[0] = s1; p[1] = s2;
@@ -884,21 +803,23 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
                 asm volatile("bar.sync 2, 256;" ::: "memory");               // smem free for the next tile
             }
         }
+        });
         if (MODE == RG_FWD && x.stats_mode == 1 && tid < N) {
             double* p = g.partials + ((size_t)blockIdx.x * N + tid) * 2;
             p[0] = acc1; p[1] = acc2;
         }
+    } else if (MODE == RG_FWD && x.stats_mode == 1 && tid < N) {      // a CTA without tiles contributes zero sums
+        double* p = g.partials + ((size_t)blockIdx.x * N + tid) * 2;
+        p[0] = 0.0; p[1] = 0.0;
     }
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tmem, tmem_cols);
 }
 
 // --------------------------------------------------------------------------------------------
 // weight gradient: dW[N,K] = sum_r dZ[r,n] * Ain[r,k],  Ain = drop(act(P*scale+shift)).
-// Both operands are staged row-major ([r][col], 128-byte column chunks, 4-row SWIZZLE_128B_BASE32B
-// atoms) and consumed as MN-major tcgen05 operands: the contraction runs over rows, 8 rows per MMA.
-// Persistent CTAs accumulate their row tiles in TMEM and write one partial per CTA.
+// The contraction runs over rows.  wgmma reads 32-bit operands K-major only, so both operands are staged
+// transposed: dZ^T [128 rows n][R rows r] and Ain^T [KP rows k][R rows r], one 128-byte SWIZZLE_128B chunk per
+// operand row (R <= 32), 8 rows r per MMA K-step.  Persistent CTAs accumulate their row tiles in registers and
+// write one partial per CTA.
 // --------------------------------------------------------------------------------------------
 struct WgradArgs {
     // normalisation backward folded in (Z2 != NULL): dZ = k1*dZ_in + k3*Z2 + k0 per (group, column); dZ_in then holds dY
@@ -921,17 +842,16 @@ struct WgradArgs {
     int round_bf16;        // PTRB200_MATH_BF16: both operands rounded to bf16
 };
 
-constexpr int WG_PRODUCERS = 512;      // 16 warps split raw fp32 tiles into hi/lo TF32 operand buffers: 8 take dZ, 8 the layer input
-constexpr int WG_THREADS = WG_PRODUCERS + 32;   // + 1 control warp: TMA bulk loads and tcgen05.mma issue
+constexpr int WG_THREADS = 512;       // four warpgroups: all stage the operands, each multiplies a quarter of the dW block
 constexpr int WG_MAX_STAGES = 4;      // raw-tile ring depth bound (TMA bulk copies in flight)
 
-// Persistent, warp-specialised, TMA-fed.  Row tiles of dZ and of the layer input are contiguous in HBM, so
-// the control warp streams them into a raw shared-memory ring with 1-D bulk copies (cp.async.bulk + mbarrier
-// complete_tx) `stages` tiles ahead.  The 8 producer warps turn a raw tile into hi/lo TF32 operand buffers
-// (double buffered) and signal `opready`; the control warp issues the MMAs of that tile (they accumulate in TMEM
-// across all tiles of the CTA), commits to `opfree`, and refills the raw slot.  No CTA-wide barrier in the loop.
+// Persistent and TMA-fed.  Row tiles of dZ and of the layer input are contiguous in HBM, so warp 0 streams them into
+// a raw shared-memory ring with 1-D bulk copies (cp.async.bulk + mbarrier complete_tx) `stages` tiles ahead.  All
+// threads turn a raw tile into transposed hi/lo TF32 operand buffers (double buffered); the MMAs of a tile run
+// asynchronously while the next tile is staged.  Warpgroup w multiplies dZ columns [64 (w & 1), +64) by the input
+// columns of half (w >> 1) of the block.
 template <int PASSES>
-__global__ void __launch_bounds__(WG_THREADS) wgrad_tc_kernel(WgradArgs g) {
+__global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(WgradArgs g) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     const int R = g.tile_rows;
@@ -940,250 +860,190 @@ __global__ void __launch_bounds__(WG_THREADS) wgrad_tc_kernel(WgradArgs g) {
     const int N = min(128, g.N_full - m0), K = min(g.kb, g.K_full - kk0), KP = ((K + 15) / 16) * 16;
     const int Nmax = min(128, g.N_full), Kmax = min(g.kb, g.K_full);       // buffer geometry is the same in every CTA
     const bool blocked = gridDim.y > 1 || gridDim.z > 1;
-    const int z_chunks = 4;                                  // dZ columns padded to 128 (MMA M = 128)
-    const int p_chunks = (((Kmax + 15) / 16) * 16 + 31) / 32;
-    const int chunk_bytes = R * 128;
-    const int op_bytes = (z_chunks + p_chunks) * chunk_bytes * (PASSES == 3 ? 2 : 1);
+    const int KPmax = ((Kmax + 15) / 16) * 16;
+    const int zop_bytes = 128 * 128, pop_bytes = KPmax * 128;  // one 128-byte chunk (32 rows r) per operand row
+    const int op_bytes = (zop_bytes + pop_bytes) * (PASSES == 3 ? 2 : 1);
     const bool fused_dz = g.Z2 != nullptr;
     const int rawz1 = ((R * Nmax * 4 + 127) / 128) * 128;
     const int rawz_bytes = rawz1 * (fused_dz ? 2 : 1), rawp_bytes = ((R * Kmax * 4 + 127) / 128) * 128;   // [dY | Z2] then the layer input
     const int stages = g.stages;
-    unsigned char* opbuf = base;                             // [2][op_bytes]
+    unsigned char* opbuf = base;                             // [2][dZ hi | dZ lo | P hi | P lo]
     unsigned char* rawbuf = opbuf + 2 * op_bytes;            // [stages][rawz + rawp]
     unsigned char* tail = rawbuf + stages * (rawz_bytes + rawp_bytes);
     uint64_t* full = reinterpret_cast<uint64_t*>(tail);      // [stages] raw tile landed (TMA complete_tx)
-    uint64_t* opready = full + WG_MAX_STAGES;                // [2] operand buffer staged (one arrive per producer warp)
-    uint64_t* opfree = opready + 2;                          // [2] MMAs reading the operand buffer have completed
-    uint32_t* slot = reinterpret_cast<uint32_t*>(opfree + 2);
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int KPmax = ((Kmax + 15) / 16) * 16;
-    const uint32_t tmem_cols = KPmax <= 32 ? 32 : KPmax <= 64 ? 64 : KPmax <= 128 ? 128 : 256;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
     if (tid == 0) {
         for (int s = 0; s < stages; ++s) tc::mbar_init(full + s, 1);
-        for (int o = 0; o < 2; ++o) { tc::mbar_init(opready + o, WG_PRODUCERS / 32); tc::mbar_init(opfree + o, 1); }
         tc::mbar_fence_init();
     }
-    if (warp == 0) tc::tmem_alloc(slot, tmem_cols);
-    tc::fence_before_sync();
-    __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tmem = *slot;
     const int ntiles = (g.rows + R - 1) / R;
     const int my_tiles = blockIdx.x < ntiles ? (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-    const bool z_aligned = ((R * N * 4) & 15) == 0;
 
-    if (warp == WG_PRODUCERS / 32) {
-        // ======================= control warp =======================
-        // warp-uniform loop (descriptors in uniform registers); one elected lane issues TMA / MMA / commit
-        {
-            const uint32_t idesc = tc::instr_desc(2, 128, KP) | (1u << 15) | (1u << 16);   // A and B MN-major
-            const bool leader = tc::elect_one();
-            // whole-warp call: un-blocked tiles are contiguous in HBM (one copy per operand, issued by the leader);
-            // column blocks are row segments, one pair of copies per row, issued by lane = row
-            auto issue_load = [&](int it, int s) {
-                const int t = blockIdx.x + it * gridDim.x;
-                const int row0 = t * R, nrows = min(R, g.rows - row0);
-                const uint32_t zb = (uint32_t)nrows * N * 4, pb = (uint32_t)nrows * K * 4;
-                unsigned char* rz = rawbuf + s * (rawz_bytes + rawp_bytes);
-                if (!blocked) {
-                    if (leader) {
-                        if ((zb & 15) == 0) {
-                            tc::mbar_expect_tx(full + s, (fused_dz ? 2 * zb : zb) + pb);
-                            tc::bulk_g2s(rz, g.dZ + (size_t)row0 * N, zb, full + s);
-                            if (fused_dz) tc::bulk_g2s(rz + rawz1, g.Z2 + (size_t)row0 * N, zb, full + s);
-                        } else {
-                            tc::mbar_expect_tx(full + s, pb);     // odd-sized dZ tail tile: producers copy it by hand
-                        }
-                        tc::bulk_g2s(rz + rawz_bytes, g.P + (size_t)row0 * K, pb, full + s);
-                    }
+    // whole-warp call (warp 0): un-blocked tiles are contiguous in HBM (one copy per operand, issued by lane 0);
+    // column blocks are row segments, one pair of copies per row, issued by lane = row
+    auto issue_load = [&](int it, int s) {
+        const int t = blockIdx.x + it * gridDim.x;
+        const int row0 = t * R, nrows = min(R, g.rows - row0);
+        const uint32_t zb = (uint32_t)nrows * N * 4, pb = (uint32_t)nrows * K * 4;
+        unsigned char* rz = rawbuf + s * (rawz_bytes + rawp_bytes);
+        if (!blocked) {
+            if (lane == 0) {
+                if ((zb & 15) == 0) {
+                    tc::mbar_expect_tx(full + s, (fused_dz ? 2 * zb : zb) + pb);
+                    tc::bulk_g2s(rz, g.dZ + (size_t)row0 * N, zb, full + s);
+                    if (fused_dz) tc::bulk_g2s(rz + rawz1, g.Z2 + (size_t)row0 * N, zb, full + s);
                 } else {
-                    const bool z_bulk = (N & 3) == 0;            // a dZ row segment must be a multiple of 16 bytes for TMA
-                    if (leader) tc::mbar_expect_tx(full + s, (z_bulk ? zb : 0u) + pb);
-                    __syncwarp();
-                    if (lane < nrows) {
-                        if (z_bulk) tc::bulk_g2s(rz + (size_t)lane * N * 4, g.dZ + (size_t)(row0 + lane) * g.N_full + m0, (uint32_t)N * 4, full + s);
-                        tc::bulk_g2s(rz + rawz_bytes + (size_t)lane * K * 4, g.P + (size_t)(row0 + lane) * g.K_full + kk0, (uint32_t)K * 4, full + s);
-                    }
-                    __syncwarp();
+                    tc::mbar_expect_tx(full + s, pb);     // odd-sized dZ tail tile: the threads copy it by hand
                 }
-            };
-            int s_load = 0;
-            for (int it = 0; it < min(stages, my_tiles); ++it) { issue_load(it, s_load); s_load = s_load + 1 == stages ? 0 : s_load + 1; }
-            int s_cons = 0, next_load = min(stages, my_tiles);
-            const uint32_t op_base = tc::smem_u32(opbuf);
-            for (int it = 0; it < my_tiles; ++it) {
-                const int o = it & 1;
-                const int t = blockIdx.x + it * gridDim.x, nrows = min(R, g.rows - t * R);
-                tc::mbar_wait(opready + o, (it >> 1) & 1);          // operands staged => raw slot s_cons drained too
-                if (next_load < my_tiles) { issue_load(next_load, s_cons); ++next_load; }
-                s_cons = s_cons + 1 == stages ? 0 : s_cons + 1;
-                tc::fence_after_sync();
-                const uint32_t zb_hi = op_base + o * op_bytes;
-                const uint32_t zb_lo = zb_hi + z_chunks * chunk_bytes;
-                const uint32_t pb_hi = zb_hi + (PASSES == 3 ? 2 : 1) * z_chunks * chunk_bytes;
-                const uint32_t pb_lo = pb_hi + p_chunks * chunk_bytes;
-                // MN-major descriptors: leading offset = distance between 128-byte column chunks, stride = 4-row atoms;
-                // a K-step of 8 rows advances the start address by 1024 B (64 in descriptor units)
-                uint64_t zh = tc::smem_desc_sw128_mn(zb_hi, chunk_bytes, 512), ph = tc::smem_desc_sw128_mn(pb_hi, chunk_bytes, 512);
-                uint64_t zl = tc::smem_desc_sw128_mn(zb_lo, chunk_bytes, 512), pl = tc::smem_desc_sw128_mn(pb_lo, chunk_bytes, 512);
-                const int ksteps = (nrows + 7) / 8;
-                if (leader) {
-                    for (int st = 0; st < ksteps; ++st) {
-                        const uint32_t acc = (it == 0 && st == 0) ? 0u : 1u;
-                        if (PASSES == 3) {
-                            tc::mma_tf32(tmem, zl, ph, idesc, acc);
-                            tc::mma_tf32(tmem, zh, pl, idesc, 1u);
-                            tc::mma_tf32(tmem, zh, ph, idesc, 1u);
-                        } else {
-                            tc::mma_tf32(tmem, zh, ph, idesc, acc);
-                        }
-                        zh += 64; ph += 64; zl += 64; pl += 64;
-                    }
-                    tc::mma_commit(opfree + o);
-                }
-                __syncwarp();
+                tc::bulk_g2s(rz + rawz_bytes, g.P + (size_t)row0 * K, pb, full + s);
             }
-        }
-    } else {
-        // ======================= producer warps =======================
-        // 16 warps turn a raw tile into the two MN-major operands.  Everything here is issue-bound (profiles/): shared memory
-        // is addressed through 32-bit shared-space addresses (ld.shared / st.shared, no generic 64-bit pointer math), the
-        // units that are pure padding (columns beyond N resp. K) are zeroed once and never touched again, the two roles
-        // split both operands so that neither idles, and with a single statistics group (batch-level BN) the three
-        // coefficient rows of the folded normalisation backward sit in shared memory instead of being re-read per unit.
-        RowsGemmArgs pg{};
-        pg.scale = g.scale; pg.shift = g.shift; pg.act = g.act; pg.gr_prev = g.gr_prev; pg.K = g.K_full; pg.drop = g.drop;
-        const bool plain_p = !g.scale && g.act == PTRB200_AF_NONE && !g.drop.thr;   // layer input already materialised
-        const int ptid = tid & 255, role = tid >> 8;      // role 0: dZ chunks {0,3} + input chunks {0,2,..}; role 1: dZ {1,2} + input {1,3,..}
-        const int r = ptid >> 3, j = ptid & 7;            // one 16-byte unit per thread per 32-column chunk (R*8 <= 256)
-        const bool vec_z = (N & 3) == 0;
-        const bool active = ptid < R * 8;
-        const uint32_t sw = tc::swz32_offset(r, j);       // this thread's slot inside every operand chunk
-        const uint32_t op_s = tc::smem_u32(opbuf), raw_s = tc::smem_u32(rawbuf), coef_s = tc::smem_u32(tail) + 128u;
-        const uint32_t stage_bytes = (uint32_t)(rawz_bytes + rawp_bytes);
-        const uint32_t zsrc_off = (uint32_t)(r * N + j * 4) * 4u, psrc_off = (uint32_t)rawz_bytes + (uint32_t)(r * K + j * 4) * 4u;
-        const uint32_t z_lo_off = (uint32_t)(z_chunks * chunk_bytes);
-        const uint32_t p_hi_off = (uint32_t)((PASSES == 3 ? 2 : 1) * z_chunks * chunk_bytes), p_lo_off = p_hi_off + (uint32_t)(p_chunks * chunk_bytes);
-        const bool single_group = fused_dz && g.gr_cur >= g.rows;
-        {   // padding units are zero for the whole kernel; the coefficient rows of the one statistics group are staged once
-            for (int e = tid; e < 2 * op_bytes / 16; e += WG_PRODUCERS) tc::sts128(op_s + (uint32_t)e * 16u, make_float4(0.f, 0.f, 0.f, 0.f));
-            if (single_group)
-                for (int e = tid; e < 3 * 128; e += WG_PRODUCERS) {
-                    const int which = e >> 7, n = e & 127;
-                    const float* src = which == 0 ? g.kc1 : which == 1 ? g.kc3 : g.kc0;
-                    reinterpret_cast<float*>(tail + 128)[e] = n < N ? __ldg(src + m0 + n) : 0.0f;
-                }
-            asm volatile("bar.sync 1, %0;" ::"n"(WG_PRODUCERS) : "memory");
-        }
-        auto put = [&](uint32_t hi_addr, uint32_t lo_addr, float4 v) {
-            if (PASSES == 3) {
-                float4 h, l;
-                tc::split_tf32(v.x, h.x, l.x); tc::split_tf32(v.y, h.y, l.y); tc::split_tf32(v.z, h.z, l.z); tc::split_tf32(v.w, h.w, l.w);
-                tc::sts128(hi_addr, h); tc::sts128(lo_addr, l);
-            } else {
-                if (g.round_bf16) v = make_float4(bf16_rn(v.x), bf16_rn(v.y), bf16_rn(v.z), bf16_rn(v.w));
-                tc::sts128(hi_addr, v);
-            }
-        };
-        int s = 0;
-        for (int it = 0; it < my_tiles; ++it) {
-            const int t = blockIdx.x + it * gridDim.x, o = it & 1;
-            const int row0 = t * R, nrows = min(R, g.rows - row0);
-            const uint32_t zb = op_s + (uint32_t)(o * op_bytes) + sw;       // this thread's slot in chunk 0 of the dZ (hi) operand
-            const uint32_t rbase = raw_s + (uint32_t)s * stage_bytes;
-            float* rz = reinterpret_cast<float*>(rawbuf + s * (rawz_bytes + rawp_bytes));
-            uint64_t* fbar = full + s;
-            const int fpar = (it / stages) & 1;
-            s = s + 1 == stages ? 0 : s + 1;
-            if (it >= 2) tc::mbar_wait(opfree + o, ((it - 2) >> 1) & 1);    // MMAs of tile it-2 are done with this buffer
-            if (blocked ? (N & 3) != 0 : (((uint32_t)nrows * N * 4) & 15) != 0) {   // dZ not TMA-sized: copy by hand, producers only
-                for (int e = tid; e < nrows * N; e += WG_PRODUCERS) rz[e] = g.dZ[(size_t)(row0 + e / N) * g.N_full + m0 + e % N];
-                asm volatile("bar.sync 1, %0;" ::"n"(WG_PRODUCERS) : "memory");
-            }
-            tc::mbar_wait(fbar, fpar);
-            const bool row_ok = r < nrows;
-            if (active) {
-                // ---- dZ operand: two of the four 32-column chunks ----
-                const size_t grp_off = (fused_dz && !single_group) ? (size_t)((row0 + r) / g.gr_cur) * g.N_full + m0 : 0;   // one division per tile
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int ch = role == 0 ? (h == 0 ? 0 : 3) : (h == 0 ? 1 : 2);
-                    const int n = ch * 32 + j * 4;
-                    if (n < N) {
-                        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (row_ok) {
-                            const uint32_t src = rbase + zsrc_off + (uint32_t)ch * 128u;
-                            if (vec_z) v = tc::lds128(src);
-                            else { v.x = tc::lds32(src); if (n + 1 < N) v.y = tc::lds32(src + 4); if (n + 2 < N) v.z = tc::lds32(src + 8); if (n + 3 < N) v.w = tc::lds32(src + 12); }
-                            if (fused_dz) {                            // host guarantees N % 4 == 0 here
-                                const float4 z = tc::lds128(src + (uint32_t)rawz1);
-                                float4 a1, a3, a0;
-                                if (single_group) {
-                                    a1 = tc::lds128(coef_s + (uint32_t)n * 4u); a3 = tc::lds128(coef_s + 512u + (uint32_t)n * 4u); a0 = tc::lds128(coef_s + 1024u + (uint32_t)n * 4u);
-                                } else {
-                                    a1 = __ldg(reinterpret_cast<const float4*>(g.kc1 + grp_off + n));
-                                    a3 = __ldg(reinterpret_cast<const float4*>(g.kc3 + grp_off + n));
-                                    a0 = __ldg(reinterpret_cast<const float4*>(g.kc0 + grp_off + n));
-                                }
-                                v.x = fmaf(a1.x, v.x, fmaf(a3.x, z.x, a0.x)); v.y = fmaf(a1.y, v.y, fmaf(a3.y, z.y, a0.y));
-                                v.z = fmaf(a1.z, v.z, fmaf(a3.z, z.z, a0.z)); v.w = fmaf(a1.w, v.w, fmaf(a3.w, z.w, a0.w));
-                            }
-                        }
-                        put(zb + (uint32_t)(ch * chunk_bytes), zb + z_lo_off + (uint32_t)(ch * chunk_bytes), v);
-                    }
-                }
-                // ---- layer-input operand: every other chunk ----
-                for (int ch = role; ch < p_chunks; ch += 2) {
-                    const int k = ch * 32 + j * 4;
-                    if (k < K) {
-                        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (row_ok) {
-                            v = tc::lds128(rbase + psrc_off + (uint32_t)ch * 128u);
-                            if (!plain_p) v = prologue4(pg, v, row0 + r, kk0 + k, true, (g.scale && g.gr_prev < g.rows) ? (size_t)((row0 + r) / g.gr_prev) * g.K_full : 0);
-                        }
-                        put(zb + p_hi_off + (uint32_t)(ch * chunk_bytes), zb + p_lo_off + (uint32_t)(ch * chunk_bytes), v);
-                    }
-                }
-            }
-            tc::fence_proxy_async();                       // this thread's operand stores -> visible to the MMA (async proxy)
+        } else {
+            const bool z_bulk = (N & 3) == 0;            // a dZ row segment must be a multiple of 16 bytes for TMA
+            if (lane == 0) tc::mbar_expect_tx(full + s, (z_bulk ? zb : 0u) + pb);
             __syncwarp();
-            if (lane == 0) tc::mbar_arrive(opready + o);
-        }
-        (void)z_aligned;
-    }
-    // ---- epilogue (producer warps 0..7): this CTA's partial dW[n][k], n = TMEM lane ----
-    if (warp < WG_PRODUCERS / 32) {
-        if (my_tiles >= 1) { const int it = my_tiles - 1; tc::mbar_wait(opfree + (it & 1), (it >> 1) & 1); }
-        tc::fence_after_sync();
-        constexpr int NSPLIT = WG_PRODUCERS / 128;           // warps per TMEM lane quarter: each takes a column range
-        const int q = warp & 3, part = warp >> 2;
-        const int n = q * 32 + lane;
-        float* dst = g.partials + (size_t)blockIdx.x * g.N_full * g.K_full + (size_t)m0 * g.K_full + kk0;
-        const int cols_part = ((KP / 8 + NSPLIT - 1) / NSPLIT) * 8;
-        const int c_begin = min(part * cols_part, KP), c_end = min(c_begin + cols_part, KP);
-        for (int c0 = c_begin; c0 < c_end; c0 += 8) {
-            float v[8];
-            if (my_tiles > 0) tc::tmem_ld8(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-            else {
-#pragma unroll
-                for (int e = 0; e < 8; ++e) v[e] = 0.0f;
+            if (lane < nrows) {
+                if (z_bulk) tc::bulk_g2s(rz + (size_t)lane * N * 4, g.dZ + (size_t)(row0 + lane) * g.N_full + m0, (uint32_t)N * 4, full + s);
+                tc::bulk_g2s(rz + rawz_bytes + (size_t)lane * K * 4, g.P + (size_t)(row0 + lane) * g.K_full + kk0, (uint32_t)K * 4, full + s);
             }
-            if (n < N) {
-                float* drow = dst + (size_t)n * g.K_full + c0;
-                if (c0 + 8 <= K && ((g.K_full | kk0) & 3) == 0 && (reinterpret_cast<uintptr_t>(g.partials) & 15) == 0) {
-                    *reinterpret_cast<float4*>(drow) = make_float4(v[0], v[1], v[2], v[3]);
-                    *reinterpret_cast<float4*>(drow + 4) = make_float4(v[4], v[5], v[6], v[7]);
-                } else {
+            __syncwarp();
+        }
+    };
+
+    const bool plain_p = !g.scale && g.act == PTRB200_AF_NONE && !g.drop.thr;   // layer input already materialised
+    const bool single_group = fused_dz && g.gr_cur >= g.rows;
+    float* coef = reinterpret_cast<float*>(tail + 128);      // [3][128] k1 | k3 | k0 of the one statistics group
+    {   // padding (columns beyond N resp. K, rows r beyond R) is zero for the whole kernel; the coefficient rows of the
+        // one statistics group are staged once
+        const uint32_t op_s = tc::smem_u32(opbuf);
+        for (int e = tid; e < 2 * op_bytes / 16; e += WG_THREADS) tc::sts128(op_s + (uint32_t)e * 16u, make_float4(0.f, 0.f, 0.f, 0.f));
+        if (single_group)
+            for (int e = tid; e < 3 * 128; e += WG_THREADS) {
+                const int which = e >> 7, n = e & 127;
+                const float* src = which == 0 ? g.kc1 : which == 1 ? g.kc3 : g.kc0;
+                coef[e] = n < N ? __ldg(src + m0 + n) : 0.0f;
+            }
+        __syncthreads();
+    }
+    if (warp == 0)
+        for (int it = 0; it < min(stages, my_tiles); ++it) issue_load(it, it);
+
+    auto put = [&](unsigned char* hi, unsigned char* lo, uint32_t off, float4 v) {
+        if (PASSES == 3) {
+            float4 h, l;
+            tc::split_tf32(v.x, h.x, l.x); tc::split_tf32(v.y, h.y, l.y); tc::split_tf32(v.z, h.z, l.z); tc::split_tf32(v.w, h.w, l.w);
+            *reinterpret_cast<float4*>(hi + off) = h;
+            *reinterpret_cast<float4*>(lo + off) = l;
+        } else {
+            if (g.round_bf16) v = make_float4(bf16_rn(v.x), bf16_rn(v.y), bf16_rn(v.z), bf16_rn(v.w));
+            *reinterpret_cast<float4*>(hi + off) = v;
+        }
+    };
+    // warpgroup tile: dZ rows [64 mh, +64) x input columns [c0, c0 + KPh).  Both column halves have the same compile-time
+    // width KPh = ceil(KP / 32) * 16: the second starts at KP - KPh (overlapping the first by at most 16 columns, which it
+    // computes but does not write), so no operand row beyond KP is read
+    const int mh = wg & 1, KPh = ((KP / 16 + 1) / 2) * 16, c0 = (wg >> 1) ? KP - KPh : 0, cw0 = (wg >> 1) ? KPh : 0;
+    const int RQ = R / 4;                                    // 16-byte units (4 rows r) per operand row
+
+    tc::with_width(KPh, [&](auto W) {
+    constexpr int NPc = decltype(W)::value;
+    float acc[NPc / 2];
 #pragma unroll
-                    for (int e = 0; e < 8; ++e) if (c0 + e < K) drow[e] = v[e];
+    for (int e = 0; e < NPc / 2; ++e) acc[e] = 0.0f;
+    for (int it = 0; it < my_tiles; ++it) {
+        const int t = blockIdx.x + it * gridDim.x, o = it & 1, s = it % stages;
+        const int row0 = t * R, nrows = min(R, g.rows - row0);
+        const float* rz = reinterpret_cast<const float*>(rawbuf + s * (rawz_bytes + rawp_bytes));
+        const float* rp = reinterpret_cast<const float*>(rawbuf + s * (rawz_bytes + rawp_bytes) + rawz_bytes);
+        if (blocked ? (N & 3) != 0 : (((uint32_t)nrows * N * 4) & 15) != 0) {   // dZ not TMA-sized: copy by hand
+            float* rzw = const_cast<float*>(rz);
+            for (int e = tid; e < nrows * N; e += WG_THREADS) rzw[e] = g.dZ[(size_t)(row0 + e / N) * g.N_full + m0 + e % N];
+            __syncthreads();
+        }
+        tc::mbar_wait(full + s, (it / stages) & 1);
+        unsigned char* zh = opbuf + o * op_bytes;
+        unsigned char* zl = zh + zop_bytes;
+        unsigned char* ph = zh + (PASSES == 3 ? 2 : 1) * zop_bytes;
+        unsigned char* pl = ph + pop_bytes;
+        // ---- dZ^T: unit (n, q) = dZ[4q .. 4q+3][n] ----
+        for (int u = tid; u < 128 * RQ; u += WG_THREADS) {
+            const int n = u & 127, qq = u >> 7;
+            if (n >= N) continue;
+            float v[4];
+            const size_t grp_off_base = (size_t)m0 + n;
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int r = qq * 4 + e;
+                float x = 0.0f;
+                if (r < nrows) {
+                    x = rz[r * N + n];
+                    if (fused_dz) {                                  // host guarantees N % 4 == 0 here
+                        const float z = rz[rawz1 / 4 + r * N + n];
+                        float a1, a3, a0;
+                        if (single_group) { a1 = coef[n]; a3 = coef[128 + n]; a0 = coef[256 + n]; }
+                        else {
+                            const size_t go = (size_t)((row0 + r) / g.gr_cur) * g.N_full + grp_off_base;
+                            a1 = __ldg(g.kc1 + go); a3 = __ldg(g.kc3 + go); a0 = __ldg(g.kc0 + go);
+                        }
+                        x = fmaf(a1, x, fmaf(a3, z, a0));
+                    }
                 }
+                v[e] = x;
             }
+            put(zh, zl, tc::swz_offset(n, qq), make_float4(v[0], v[1], v[2], v[3]));
         }
+        // ---- layer input^T: unit (k, q) = Ain[4q .. 4q+3][k] ----
+        for (int u = tid; u < KP * RQ; u += WG_THREADS) {
+            const int k = u % KP, qq = u / KP;
+            if (k >= K) continue;
+            float v[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int r = qq * 4 + e;
+                float x = 0.0f;
+                if (r < nrows) {
+                    x = rp[r * K + k];
+                    if (!plain_p) {
+                        const int row = row0 + r, col = kk0 + k;
+                        if (g.scale) {
+                            const size_t co = (g.gr_prev < g.rows ? (size_t)(row / g.gr_prev) * g.K_full : 0) + col;
+                            x = fmaf(x, __ldg(g.scale + co), __ldg(g.shift + co));
+                        }
+                        if (g.act != PTRB200_AF_NONE) x = activate(g.act, x).y;
+                        if (g.drop.thr) x = dropout_keep(g.drop.key, (uint64_t)row * g.K_full + col, g.drop.thr) ? x * g.drop.scale : 0.0f;
+                    }
+                }
+                v[e] = x;
+            }
+            put(ph, pl, tc::swz_offset(k, qq), make_float4(v[0], v[1], v[2], v[3]));
+        }
+        tc::fence_proxy_async();
+        __syncthreads();
+        if (warp == 0 && it + stages < my_tiles) issue_load(it + stages, s);   // raw slot s is drained
+        const uint32_t a_s = tc::smem_u32(zh) + mh * 8192, b_s = tc::smem_u32(ph) + c0 * 128;
+        const uint64_t ah = tc::smem_desc_sw128(a_s, 1024), bh = tc::smem_desc_sw128(b_s, 1024);
+        const uint64_t al = tc::smem_desc_sw128(a_s + zop_bytes, 1024), bl = tc::smem_desc_sw128(b_s + pop_bytes, 1024);
+        // four K-steps of 8 rows r (+32 B each): rows beyond the tile are zero in the operand buffers
+        tc::wg_fence();
+#pragma unroll
+        for (int st = 0; st < 4; ++st) {
+            if (PASSES == 3) {
+                tc::mma_tf32<NPc>(acc, al + 2 * st, bh + 2 * st, 1u);
+                tc::mma_tf32<NPc>(acc, ah + 2 * st, bl + 2 * st, 1u);
+            }
+            tc::mma_tf32<NPc>(acc, ah + 2 * st, bh + 2 * st, 1u);
+        }
+        tc::wg_commit();
+        tc::wg_wait<0>();                                    // the same threads stage the next tile
     }
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tmem, tmem_cols);
+    // ---- epilogue: this CTA's partial dW[n][k] ----
+    float* dst = g.partials + (size_t)blockIdx.x * g.N_full * g.K_full + (size_t)m0 * g.K_full + kk0;
+#pragma unroll
+    for (int e = 0; e < NPc / 2; ++e) {
+        const int n = mh * 64 + tc::acc_row(e), k = c0 + tc::acc_col(e);
+        if (n < N && k >= cw0 && k < K) dst[(size_t)n * g.K_full + k] = acc[e];
+    }
+    });
 }
 
 }  // namespace ptrb200

@@ -1,18 +1,20 @@
-// tc.cuh -- thin inline-PTX layer over the sm_100a tensor-core path:
-// tcgen05.mma (kind::tf32 / kind::f16) with shared-memory operand descriptors, TMEM allocation
-// and loads, mbarrier completion, and the 128B-swizzled K-major operand layout.
+// tc.cuh -- thin inline-PTX layer over the sm_90a tensor-core path:
+// wgmma.mma_async (tf32, fp32 accumulators in registers) with shared-memory operand descriptors,
+// mbarrier completion, 1-D TMA bulk copies, and the 128B-swizzled K-major operand layout.
 //
 // Operand layout ("K-major, SWIZZLE_128B"): an operand tile of R rows (R % 8 == 0) is cut along
-// K into chunks of 128 bytes (32 tf32 / 64 bf16).  One chunk is R rows x 128 B stored as 8-row
-// atoms of 1024 B; inside an atom the 16-byte unit j of row r sits at unit (j ^ (r & 7)).
-// A chunk base must be 1024-byte aligned.  One tcgen05.mma consumes 32 bytes of K per row, so a
-// chunk feeds 4 MMA K-steps; step s starts 32*s bytes into the chunk (descriptor start address).
+// K into chunks of 128 bytes (32 tf32).  One chunk is R rows x 128 B stored as 8-row atoms of
+// 1024 B; inside an atom the 16-byte unit j of row r sits at unit (j ^ (r & 7)).  A chunk base must
+// be 1024-byte aligned.  One wgmma consumes 32 bytes of K per row, so a chunk feeds 4 MMA K-steps;
+// step s starts 32*s bytes into the chunk (descriptor start address).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 namespace ptrb200 {
 namespace tc {
+
+template <int N> struct WidthT { static constexpr int value = N; };
 
 constexpr int CHUNK_BYTES = 128;            // K extent of one swizzle atom row
 constexpr int ATOM_BYTES = 1024;            // 8 rows x 128 B
@@ -67,15 +69,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity) {
     while (!mbar_try_wait(bar, parity)) { __nanosleep(40); }
 }
-// true in exactly one lane of a fully converged warp (keeps the surrounding control flow warp-uniform, so
-// descriptors stay in uniform registers instead of being moved lane -> uniform before every tcgen05.mma)
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-
-// generic-proxy smem writes -> visible to the async proxy (tcgen05.mma operand reads, bulk copies)
+// generic-proxy smem writes -> visible to the async proxy (wgmma operand reads, bulk copies)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---- bulk async copy (TMA engine, 1-D): global -> shared, completion on an mbarrier -------------
@@ -94,88 +88,124 @@ __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.w
 template <int N>
 __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 
-// ---- TMEM ----------------------------------------------------------------------
-// one full warp allocates `cols` (power of two >= 32) TMEM columns; base address lands in *slot
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t base, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(base), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// 32 lanes x 8 consecutive fp32 columns: thread t of the warp receives lane (lane_base + t)
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float (&v)[8]) {
-    uint32_t r0, r1, r2, r3, r4, r5, r6, r7;
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3), "=r"(r4), "=r"(r5), "=r"(r6), "=r"(r7) : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-    v[0] = __uint_as_float(r0); v[1] = __uint_as_float(r1); v[2] = __uint_as_float(r2); v[3] = __uint_as_float(r3);
-    v[4] = __uint_as_float(r4); v[5] = __uint_as_float(r5); v[6] = __uint_as_float(r6); v[7] = __uint_as_float(r7);
-}
-// 32 lanes x 16 columns
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// ---- descriptors -----------------------------------------------------------------
-// shared-memory operand descriptor: K-major, SWIZZLE_128B, 8-row atoms `sbo_bytes` apart
+// ---- warpgroup MMA (wgmma) ------------------------------------------------------------
+// shared-memory operand descriptor (sm_90 format): K-major, SWIZZLE_128B, 8-row atoms `sbo_bytes` apart.
+// A K-step of 8 tf32 (32 bytes) advances the start address by 32 bytes inside the swizzle atom.
 __device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t smem_addr, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3ffffu) >> 4);              // start address  [0,14)
-    d |= (uint64_t)1 << 16;                                     // leading byte offset (ignored for swizzled K-major) [16,30)
+    d |= (uint64_t)1 << 16;                                     // leading byte offset (unused for swizzled K-major) [16,30)
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32;          // stride byte offset [32,46)
-    d |= (uint64_t)1 << 46;                                     // descriptor version (Blackwell) [46,48)
-    d |= (uint64_t)2 << 61;                                     // layout type SWIZZLE_128B [61,64)
+    d |= (uint64_t)1 << 62;                                     // layout type SWIZZLE_128B [62,64)
     return d;
-}
-// MN-major tf32 operand (the contraction index runs over the ROWS of a row-major staged tile).
-// The only legal layout for 32-bit MN-major operands is SWIZZLE_128B_BASE32B: atoms of 4 rows x 128 B,
-// the 32-byte unit u of row r stored at unit (u ^ (r & 3)).  `lbo_bytes` = distance between consecutive
-// 128-byte blocks along M/N, `sbo_bytes` = distance between consecutive 4-row groups along K.
-__device__ __forceinline__ uint32_t swz32_offset(int r, int j16) {
-    return (uint32_t)(r * 128 + ((((j16 >> 1) ^ (r & 3)) << 5) | ((j16 & 1) << 4)));
-}
-__device__ __forceinline__ uint64_t smem_desc_sw128_mn(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3ffffu) >> 4);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)1 << 61;                                     // layout type SWIZZLE_128B_BASE32B
-    return d;
-}
-// instruction descriptor: D fp32, A/B format (0 f16, 1 bf16, 2 tf32), both K-major, M x N tile
-__host__ __device__ constexpr uint32_t instr_desc(int fmt, int M, int N) {
-    return (1u << 4) | ((uint32_t)fmt << 7) | ((uint32_t)fmt << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
 }
 
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D[64 x N] (+)= A[64 x 8] * B[N x 8]^T, tf32 operands from shared memory, fp32 accumulators in registers (N / 2 per
+// thread).  Issued by a whole warpgroup; N is a compile-time constant, so one instruction covers the whole tile width.
+// scale_d = 0 overwrites D (the first K-step of a tile), 1 accumulates.  Accumulator e of lane l in warp w (of the
+// warpgroup) holds row 16 w + l/4 + 8 ((e>>1)&1), column 8 (e>>2) + 2 (l%4) + (e&1)   (see acc_row / acc_col).
+template <int N>
+__device__ __forceinline__ void mma_tf32(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d);
+
+template <>
+__device__ __forceinline__ void mma_tf32<16>(float (&d)[8], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a_desc), "l"(b_desc), "r"(scale_d) : "memory");
 }
-__device__ __forceinline__ void mma_f16(uint32_t tmem_d, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+
+template <>
+__device__ __forceinline__ void mma_tf32<32>(float (&d)[16], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a_desc), "l"(b_desc), "r"(scale_d) : "memory");
 }
-// arrive on an mbarrier once every previously issued tcgen05.mma of this thread has completed
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+
+template <>
+__device__ __forceinline__ void mma_tf32<48>(float (&d)[24], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+        : "l"(a_desc), "l"(b_desc), "r"(scale_d) : "memory");
 }
+
+template <>
+__device__ __forceinline__ void mma_tf32<64>(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a_desc), "l"(b_desc), "r"(scale_d) : "memory");
+}
+
+template <>
+__device__ __forceinline__ void mma_tf32<80>(float (&d)[40], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n80k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39}, %40, %41, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+        : "l"(a_desc), "l"(b_desc), "r"(scale_d) : "memory");
+}
+
+template <>
+__device__ __forceinline__ void mma_tf32<96>(float (&d)[48], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47}, %48, %49, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+        : "l"(a_desc), "l"(b_desc), "r"(scale_d) : "memory");
+}
+
+template <>
+__device__ __forceinline__ void mma_tf32<112>(float (&d)[56], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %58, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n112k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55}, %56, %57, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55])
+        : "l"(a_desc), "l"(b_desc), "r"(scale_d) : "memory");
+}
+
+template <>
+__device__ __forceinline__ void mma_tf32<128>(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a_desc), "l"(b_desc), "r"(scale_d) : "memory");
+}
+
+__device__ __forceinline__ int acc_row(int e) { return 16 * ((threadIdx.x >> 5) & 3) + ((threadIdx.x & 31) >> 2) + 8 * ((e >> 1) & 1); }
+__device__ __forceinline__ int acc_col(int e) { return 8 * (e >> 2) + 2 * (threadIdx.x & 3) + (e & 1); }
+
+// Calls f(std::integral_constant<int, NP>) for the run-time tile width np (a multiple of 16, 16..128): the code that
+// holds accumulators is compiled once per width, so every wgmma has a compile-time N and fixed accumulator registers.
+template <typename F>
+__device__ __forceinline__ void with_width(int np, F&& f) {
+    switch (np) {
+        case 16: f(WidthT<16>{}); break;
+        case 32: f(WidthT<32>{}); break;
+        case 48: f(WidthT<48>{}); break;
+        case 64: f(WidthT<64>{}); break;
+        case 80: f(WidthT<80>{}); break;
+        case 96: f(WidthT<96>{}); break;
+        case 112: f(WidthT<112>{}); break;
+        default: f(WidthT<128>{}); break;
+    }
+}
+
+// element (r, k) of a K-major SWIZZLE_128B chunk: the byte offset of one fp32 (an MN-major source is transposed
+// into the K-major layout with these scalar stores: wgmma reads 32-bit operands K-major only)
+__device__ __forceinline__ uint32_t swz_elem(int r, int k) { return swz_offset(r, k >> 2) + (uint32_t)((k & 3) << 2); }
 
 // split an fp32 value into tf32-representable hi and the fp32 remainder lo (hi + lo == x exactly)
 __device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {

@@ -4,7 +4,7 @@ The reference batches whole queries and asks every batch to hold lists of ONE le
 ``batch_size`` queries of equal ``num_docs`` (ptranking/data/data_utils.py:683-742), and with the default settings a
 query of 100+ documents travels alone (B = 1), which leaves a GPU launch-bound.  ``LengthBucketedBatches`` keeps the
 contract the kernels rely on -- uniform n per batch, labels presorted descending per query (data_utils.py:205-232) --
-but sizes B per bucket so that every batch carries about ``docs_per_batch`` documents (2^18 fills one B200; one step of
+but sizes B per bucket so that every batch carries about ``docs_per_batch`` documents (2^18 fills one H100; one step of
 the default scorer then runs at its large-batch rate).  Batches are assembled once into pinned host memory, so
 ``NeuralRanker.train`` can stream them with asynchronous copies.  Host-side only: no device work happens here.
 """

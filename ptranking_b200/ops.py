@@ -795,7 +795,7 @@ def _key_lens_ptr(B: int, device):
 
 
 class _AttentionTC(torch.autograd.Function):
-    """Tensor-core attention: batched tcgen05 GEMMs around a materialised [B*H,n,n] probability tensor."""
+    """Tensor-core attention: batched wgmma GEMMs around a materialised [B*H,n,n] probability tensor."""
 
     @staticmethod
     @_on_tensor_device
@@ -834,7 +834,7 @@ def attention(Q, K, V, n_heads: int, dropout_p: float = 0.0, seed: Optional[int]
               impl: Optional[str] = None):
     """softmax(Q K^T / sqrt(d)) [dropout] V per head; Q,K,V: [B,n,H*d].
 
-    impl: "tc" (tcgen05 3xTF32 GEMMs, default), "tc_tf32" (single-pass TF32), "simt" (flash-style fp32 FMA kernels);
+    impl: "tc" (wgmma 3xTF32 GEMMs, default), "tc_tf32" (single-pass TF32), "simt" (flash-style fp32 FMA kernels);
     None reads PTRANKING_B200_ATTN.  All three draw the same dropout stream."""
     if seed is None:
         seed = torch.initial_seed() & (2 ** 64 - 1)

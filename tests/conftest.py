@@ -10,12 +10,12 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
     """gpu-marked tests need a CUDA device; without one they are skipped, so a plain `pytest` on a CPU machine is
-    green instead of failing inside torch._C._cuda_init.  On a GPU box nothing is skipped: a missing
+    green instead of failing inside torch._C._cuda_init.  On a GPU machine nothing is skipped: a missing
     libptranking_b200.so must fail loudly there (there is no fallback path to hide behind)."""
     import torch
     if not torch.cuda.is_available():

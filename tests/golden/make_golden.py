@@ -1,6 +1,6 @@
 """Generate the golden fixtures in this directory by running the UNMODIFIED reference.
 
-Run in the authoring container only (the GPU box has no /root/reference):
+Run where a checkout of the reference is available (PTRANKING_REFERENCE names it):
 
     PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
 

@@ -132,7 +132,7 @@ TC_CASES = [
 
 @pytest.mark.parametrize("case", TC_CASES, ids=[f"tc{i}" for i in range(len(TC_CASES))])
 def test_tensor_core_path_matches_simt_path(case):
-    """The tcgen05 (3xTF32) layer kernels against the fp32 SIMT kernels on identical inputs,
+    """The wgmma (3xTF32) layer kernels against the fp32 SIMT kernels on identical inputs,
     dropout streams included: forward scores, parameter gradients and dX."""
     from ptranking_b200 import ops
     B, n, dims, AF, TL, norm, affine, p = case

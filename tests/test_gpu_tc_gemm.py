@@ -1,4 +1,4 @@
-"""tcgen05 GEMM building block vs a float64 matmul: 3xTF32 restores fp32-level accuracy, 1xTF32 does not."""
+"""wgmma GEMM building block vs a float64 matmul: 3xTF32 restores fp32-level accuracy, 1xTF32 does not."""
 import ctypes as C
 
 import numpy as np
@@ -42,7 +42,7 @@ def test_tc_gemm_matches_float64(shape):
 
 @pytest.mark.parametrize("shape", [(32, 100, 136), (64, 8, 32), (1000, 100, 100), (4096, 1, 100), (37, 128, 256), (5000, 100, 136)])
 def test_tc_wgrad_matches_float64(shape):
-    """dW = dZ^T P through MN-major (SWIZZLE_128B_BASE32B) tcgen05 operands."""
+    """dW = dZ^T P through operands transposed into K-major wgmma tiles while they are staged."""
     from ptranking_b200 import _lib
     lib = _lib.load()
     rows, N, K = shape

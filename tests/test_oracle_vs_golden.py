@@ -9,6 +9,18 @@ from oracle import closed_form as cf
 from oracle import ref_port as rp
 from tests.helpers import load, loss_cases, parse_loss_key, rel_err
 
+
+@pytest.fixture(autouse=True)
+def _one_intra_op_thread():
+    """Some fixture gradients are pure rounding noise (a bias feeding a BatchNorm has an exact gradient of zero), and
+    ATen's CPU reductions split their work by thread count: the oracle runs on one thread so its summation order, and
+    therefore its noise, is the same on every machine."""
+    n = torch.get_num_threads()
+    torch.set_num_threads(1)
+    yield
+    torch.set_num_threads(n)
+
+
 CASES = loss_cases()
 
 

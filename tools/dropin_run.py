@@ -2,10 +2,11 @@
 ltr.py:568 -> point_run -> kfold_cv_eval :291-369) constructs, trains, validates, checkpoints, reloads and tests the
 ptranking_b200 classes that ptranking_b200.install() registered in its module globals (ltr.py:166-171).
 
-    python tools/dropin_run.py --impl b200 --model LambdaRank [--sf pointsf|listsf]      # on a B200 box
+    python tools/dropin_run.py --impl b200 --model LambdaRank [--sf pointsf|listsf]      # on an H100
     python tools/dropin_run.py --impl reference --cuda none --model LambdaRank           # the reference itself, CPU
 
-The reference is imported from baseline/_ref (pip --target install of /root/reference, DESIGN.md section 8).  Data: synthetic
+The reference is imported from baseline/_ref (a pip --target install of wildltr/ptranking, DESIGN.md section 8) or from
+the checkout named by PTRANKING_REFERENCE.  Data: synthetic
 LETOR-format files shaped like MSLR-WEB30K (136 features, grades 0-4 with the dataset's marginals, features weakly
 informative so that learning shows) written to a scratch directory in the layout the loader expects
 (<dir>/Fold{k}/{train,vali,test}.txt, ptranking/data/data_utils.py:553-640).  debug=True: 2 folds x 5 epochs, nDCG@5 validation.
@@ -19,7 +20,7 @@ import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-for cand in (os.path.join(ROOT, "baseline", "_ref"), "/root/reference"):
+for cand in (os.path.join(ROOT, "baseline", "_ref"), os.environ.get("PTRANKING_REFERENCE", "")):
     if os.path.isdir(os.path.join(cand, "ptranking")):
         sys.path.insert(0, cand)
         REF = cand

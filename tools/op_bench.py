@@ -149,7 +149,7 @@ for L in (3, 6):
 
 os.makedirs("profiles", exist_ok=True)
 with open(f"profiles/{tag}_op_table.md", "w") as f:
-    f.write(f"# {tag}: per-op timings on one B200 (CUDA events, 20 warm iterations; `tools/op_bench.py`)\n\n")
+    f.write(f"# {tag}: per-op timings on one {torch.cuda.get_device_name()} (CUDA events, 20 warm iterations; `tools/op_bench.py`)\n\n")
     f.write("GB/s = ALGORITHMIC bytes (12n per query for a loss, n(4F+8) for the scorer) / time; frac = of the measured copy bandwidth "
             f"({HBM:.0f} GB/s).  For the list scorer the last-but-one column is GFLOP/s (algorithmic fwd+bwd FLOPs).\n\n")
     f.write("| op | shape | ms | queries/s | GB/s (GFLOP/s) | frac of HBM |\n|---|---|---|---|---|---|\n")

@@ -1,4 +1,4 @@
-"""Achieved parity errors on the GPU box -> profiles/<tag>_parity_table.md (VERDICT r1 item 1e).
+"""Achieved parity errors on the GPU -> profiles/<tag>_parity_table.md (VERDICT r1 item 1e).
 
 For every loss x n in {32, 256, 512, 1024} and every pointwise-scorer configuration: the error of the CUDA path against
 (i) the oracle = the reference's own fp32 ATen ops on the CPU, (ii) float64 truth (closed forms for the losses, the oracle
@@ -131,7 +131,7 @@ for name, over in cfgs.items():
 
 os.makedirs("profiles", exist_ok=True)
 with open(f"profiles/{tag}_parity_table.md", "w") as f:
-    f.write(f"# {tag}: achieved parity errors on one B200 (`python tools/parity_table.py`, through the C ABI)\n\n")
+    f.write(f"# {tag}: achieved parity errors on one {torch.cuda.get_device_name()} (`python tools/parity_table.py`, through the C ABI)\n\n")
     f.write("Three numbers per cell: maxabs / l2 / elem (definitions in the tool's docstring).  B = 8 queries per loss case; scores are\n"
             "sigmoid outputs (the default scorer's tail), labels follow the MSLR-WEB30K marginals, presorted.  north_star's bar: loss and\n"
             "gradient within 1e-5 relative fp32 of the reference; where the reference itself sits further than that from float64\n"

@@ -1,6 +1,6 @@
-"""SASS census of libptranking_b200.so: per kernel, the counts of the Blackwell-specific instructions that prove which
-hardware paths the binary uses (tcgen05.mma = UTCHMMA, tcgen05.ld = LDTM, TMA bulk copy = UBLKCP, tcgen05.commit = UTCBAR,
-mbarrier = SYNCS, SFU = MUFU) -> profiles/<tag>_sass_census.md.  Runs without a GPU:  python tools/sass_census.py [tag]"""
+"""SASS census of libptranking_b200.so: per kernel, the counts of the Hopper-specific instructions that prove which
+hardware paths the binary uses (wgmma.mma_async = HGMMA, wgmma.fence = WARPGROUP, TMA bulk copy = UBLKCP, mbarrier = SYNCS,
+SFU = MUFU) -> profiles/<tag>_sass_census.md.  Runs without a GPU:  python tools/sass_census.py [tag]"""
 import collections
 import os
 import re
@@ -11,7 +11,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "ptranking_b200", "lib", "libptranking_b200.so")
 tag = sys.argv[1] if len(sys.argv) > 1 else "r02"
 out = subprocess.run(["cuobjdump", "-sass", LIB], capture_output=True, text=True).stdout
-WANT = ["UTCHMMA", "LDTM", "UBLKCP", "UTCBAR", "SYNCS", "MUFU", "SHFL", "STS", "LDG", "STG"]
+WANT = ["HGMMA", "WARPGROUP", "UBLKCP", "SYNCS", "MUFU", "SHFL", "STS", "LDG", "STG"]
 kern, counts, size = None, collections.OrderedDict(), {}
 for line in out.splitlines():
     m = re.match(r"\s*Function : (\S+)", line)
@@ -32,12 +32,12 @@ rows = []
 for k, d in zip(counts, dem):
     short = re.sub(r"\(.*", "", d.replace("ptrb200::", "").replace("void ", ""))[:64]
     rows.append((short, size[k], counts[k]))
-rows.sort(key=lambda r: (-r[2]["UTCHMMA"], -r[1]))
+rows.sort(key=lambda r: (-r[2]["HGMMA"], -r[1]))
 os.makedirs(os.path.join(ROOT, "profiles"), exist_ok=True)
 path = os.path.join(ROOT, "profiles", f"{tag}_sass_census.md")
 with open(path, "w") as f:
-    f.write(f"# {tag}: SASS census of libptranking_b200.so (`cuobjdump -sass`, sm_100a; `python tools/sass_census.py`)\n\n")
-    f.write("UTCHMMA = tcgen05.mma, LDTM = tcgen05.ld (TMEM -> registers), UBLKCP = cp.async.bulk (TMA engine), UTCBAR = tcgen05.commit,\n"
+    f.write(f"# {tag}: SASS census of libptranking_b200.so (`cuobjdump -sass`, sm_90a; `python tools/sass_census.py`)\n\n")
+    f.write("HGMMA = wgmma.mma_async, WARPGROUP = wgmma fences / waits, UBLKCP = cp.async.bulk (TMA engine),\n"
             "SYNCS = mbarrier ops, MUFU = special-function unit.  Static instruction counts per kernel (not executed counts).\n\n")
     f.write("| kernel | SASS instr | " + " | ".join(WANT) + " |\n|---|---|" + "---|" * len(WANT) + "\n")
     tot = collections.Counter()
