@@ -12,7 +12,6 @@
 // Layout in HBM: activations are dense row-major [rows = B*n, width] fp32.  Per layer the
 // workspace keeps Z (pre-normalisation Linear output), A (post-activation) and, when a norm
 // is present, mean/rstd per (group, channel); group = whole batch (BN) or one query (BN2).
-#include <stdlib.h>
 #include "common.cuh"
 #include "ffnet_act.cuh"
 #include "ffnet_tc.cuh"
@@ -378,15 +377,10 @@ static void launch_colstat(cudaStream_t st, const char* tag, const float* Z, con
         const int Q = C / 4;
         int RY = 256 / Q; if (RY < 1) RY = 1; if (RY > 16) RY = 16;
         const size_t sm = (size_t)RY * Q * 8 * sizeof(double);
-        static const bool no_pf = getenv("PTRB200_NO_CS_PREFETCH") && getenv("PTRB200_NO_CS_PREFETCH")[0] == '1';   // A/B switch
-        if (WHAT == STAT_DY && nr.act == PTRB200_AF_GELU && !no_pf)
+        if (WHAT == STAT_DY && nr.act == PTRB200_AF_GELU)
             PTRB200_LAUNCH_TAG(tag, (colstat4_kernel<WHAT, PTRB200_AF_GELU, true>), grid, dim3(Q, RY), sm, st, Z, dA, dY, nr, part, gr, C, S, slice_rows, r1);
-        else if (WHAT == STAT_DY && nr.act == PTRB200_AF_RELU && !no_pf)
-            PTRB200_LAUNCH_TAG(tag, (colstat4_kernel<WHAT, PTRB200_AF_RELU, true>), grid, dim3(Q, RY), sm, st, Z, dA, dY, nr, part, gr, C, S, slice_rows, r1);
-        else if (WHAT == STAT_DY && nr.act == PTRB200_AF_GELU)
-            PTRB200_LAUNCH_TAG(tag, (colstat4_kernel<WHAT, PTRB200_AF_GELU>), grid, dim3(Q, RY), sm, st, Z, dA, dY, nr, part, gr, C, S, slice_rows, r1);
         else if (WHAT == STAT_DY && nr.act == PTRB200_AF_RELU)
-            PTRB200_LAUNCH_TAG(tag, (colstat4_kernel<WHAT, PTRB200_AF_RELU>), grid, dim3(Q, RY), sm, st, Z, dA, dY, nr, part, gr, C, S, slice_rows, r1);
+            PTRB200_LAUNCH_TAG(tag, (colstat4_kernel<WHAT, PTRB200_AF_RELU, true>), grid, dim3(Q, RY), sm, st, Z, dA, dY, nr, part, gr, C, S, slice_rows, r1);
         else
             PTRB200_LAUNCH_TAG(tag, (colstat4_kernel<WHAT, -1>), grid, dim3(Q, RY), sm, st, Z, dA, dY, nr, part, gr, C, S, slice_rows, r1);
     } else {
@@ -605,19 +599,6 @@ __global__ void norm_bwd_apply_kernel(const float* __restrict__ Z, float* __rest
     }
 }
 
-// gradients of the norm parameters from the channel totals T1 = sum dY, T2 = sum dY*xhat
-__global__ void norm_param_grad_kernel(NormRef nr, const float* __restrict__ T1, const float* __restrict__ T2,
-                                       float* dgamma, float* dbeta, float* daff_w, float* daff_b, int C) {
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= C) return;
-    const float ga = nr.gamma ? nr.gamma[c] : 1.0f, be = nr.beta ? nr.beta[c] : 0.0f;
-    const float w = nr.aff_w ? nr.aff_w[c] : 1.0f;
-    if (dgamma) dgamma[c] = w * T2[c];
-    if (dbeta) dbeta[c] = w * T1[c];
-    if (daff_w) daff_w[c] = ga * T2[c] + be * T1[c];
-    if (daff_b) daff_b[c] = T1[c];
-}
-
 // ------------------------------------------------------------------ host side
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
@@ -633,11 +614,11 @@ struct Plan {
     bool use_tc;                                 // every layer fits the tensor-core kernels (else the SIMT path runs)
     int passes;                                  // 3 = 3xTF32 (fp32-equivalent), 1 = TF32
     bool bf16;                                   // single pass with every operand rounded to bf16 first
-    int tile_rows, seg_len, group_rows, tiles_per_group, ntiles, wg_grid, wg_rows;
+    int tile_rows, seg_len, group_rows, tiles_per_group, ntiles;
     int L, G, gr, S_stat, slice_rows, S_w, k_chunk;
     size_t rows;
     LayerPlan layer[PTRB200_MAX_FF_LAYERS];
-    size_t partials_off, s1_off, s2_off, t1_off, t2_off, dbuf0_off, dbuf1_off, wpart_off, k1_off, k3_off, k0_off, sync_off, total;
+    size_t partials_off, s1_off, s2_off, dbuf0_off, dbuf1_off, wpart_off, k1_off, k3_off, k0_off, sync_off, total;
     bool sync_bn;                                // batch-level BN statistics all-reduced across data-parallel ranks
     bool ragged;                                 // per-query BN2 over a ragged batch (query boundaries from prefix offsets)
     int pad_k;                                   // > 0: input width zero-padded to this multiple of 4 for the tensor-core path
@@ -664,7 +645,7 @@ static int make_plan(const ptrb200_ffnet* net, int B, int n, Plan& p, int total_
     p.L = net->num_linear;
     // total_rows > 0: a ragged batch -- B queries cut out of total_rows documents by prefix offsets, n = longest list.
     // Batch-level BN and norm-free nets see one long list of total_rows documents (the dense code path as is); per-query
-    // BN2 needs the query boundaries and takes the ragged path (forward_ragged / backward_ragged below).
+    // BN2 needs the query boundaries and normalises with the per-query bn2_ragged_* kernels below.
     p.ragged = total_rows > 0 && net->norm == PTRB200_NORM_BN2;
     p.rows = total_rows > 0 ? (size_t)total_rows : (size_t)B * n;
     p.G = net->norm == PTRB200_NORM_BN2 ? B : 1;
@@ -698,7 +679,6 @@ static int make_plan(const ptrb200_ffnet* net, int B, int n, Plan& p, int total_
             else { p.group_rows = n; p.tiles_per_group = (n + 127) / 128; p.S_stat = p.tiles_per_group; p.slice_rows = 128; }
         } else { p.slice_rows = 128; p.S_stat = (int)((p.rows + 127) / 128); }
         p.ntiles = p.group_rows > 0 ? B * p.tiles_per_group : (int)((p.rows + p.tile_rows - 1) / p.tile_rows);
-        p.wg_rows = 32; p.wg_grid = 444;
     }
     if (p.ragged && !p.use_tc) { set_error("ffnet: ragged BN2 batches need the tensor-core path (layer widths multiples of 4)"); return PTRB200_ERR_UNSUPPORTED; }
     if (p.ragged) { p.tile_rows = 128; p.seg_len = 128; p.group_rows = 0; p.tiles_per_group = 0; p.ntiles = (int)((p.rows + 127) / 128); p.S_stat = 1; p.slice_rows = (int)p.rows; }
@@ -738,8 +718,6 @@ static int make_plan(const ptrb200_ffnet* net, int B, int n, Plan& p, int total_
     p.partials_off = off; off = align_up(off + (size_t)p.G * p.S_stat * maxd * 2 * 8, 256);
     p.s1_off = off; off = align_up(off + (size_t)p.G * maxd * 4, 256);
     p.s2_off = off; off = align_up(off + (size_t)p.G * maxd * 4, 256);
-    p.t1_off = off; off = align_up(off + (size_t)maxd * 4, 256);
-    p.t2_off = off; off = align_up(off + (size_t)maxd * 4, 256);
     p.k1_off = off; off = align_up(off + (size_t)p.G * maxd * 4, 256);
     p.k3_off = off; off = align_up(off + (size_t)p.G * maxd * 4, 256);
     p.k0_off = off; off = align_up(off + (size_t)p.G * maxd * 4, 256);
@@ -859,16 +837,13 @@ static size_t wgrad_smem(int N, int K, int KP, int& R, int passes, int& stages, 
             if (fixed + st * (rawz + rawp) <= limit) return fixed + st * (rawz + rawp);
         return 0;
     };
-    // (PTRB200_WG_DEEP=1 prefers ring depth over tile height: a 24-row tile leaves a quarter of the staging threads idle,
-    //  so by default the tallest tile that fits with 2 stages wins)
-    static const bool deep = getenv("PTRB200_WG_DEEP") && getenv("PTRB200_WG_DEEP")[0] == '1';
-    for (int pass = deep ? 0 : 1; pass < 2; ++pass)
-        for (int h : heights) {
-            if (h < min_R) continue;
-            int st = 0;
-            const size_t bytes = fit(h, st);
-            if (bytes && (pass == 1 || st >= 3)) { R = h; stages = st; return bytes; }
-        }
+    // (a 24-row tile leaves a quarter of the staging threads idle, so the tallest tile that fits with 2 stages wins over depth)
+    for (int h : heights) {
+        if (h < min_R) continue;
+        int st = 0;
+        const size_t bytes = fit(h, st);
+        if (bytes) { R = h; stages = st; return bytes; }
+    }
     R = 8; stages = 2;
     return limit + 1;        // does not fit
 }
@@ -884,7 +859,6 @@ static bool rows_ws_fits(int K, int N, int passes) {
 static int launch_rows_gemm(int mode, int passes, RowsGemmArgs& g, int ntiles, cudaStream_t st,
                             int stats_kind = 0, int* S_out = nullptr, int S_default = 1) {
     g.NP = ((g.N + 15) / 16) * 16;
-    { static const int no_partial = getenv("PTRB200_NO_PARTIAL") ? 1 : 0; g.no_partial = no_partial; }
     int rc;
     const int nchunks = (g.K + 31) / 32;
     // ---- persistent warp-specialised kernel when the whole weight image fits beside the A ring ----
@@ -910,14 +884,11 @@ static int launch_rows_gemm(int mode, int passes, RowsGemmArgs& g, int ntiles, c
         }
         // the prologue activation is a template parameter for the common codes, -1 = generic run-time switch
         const int act_t = (g.act == PTRB200_AF_NONE || g.act == PTRB200_AF_RELU || g.act == PTRB200_AF_GELU || g.act == PTRB200_AF_SIGM) ? g.act : -1;
-        // width-specialised instantiations for the default scorer (136 features, 100-wide hidden layers); PTRB200_NO_KT=1 skips them
-        static const bool no_kt = getenv("PTRB200_NO_KT") != nullptr;
-        if (!no_kt) {
-            RW_CASE_K(RG_FWD, 3, PTRB200_AF_NONE, 136, "rows_gemm_ws_fwd") RW_CASE_K(RG_FWD, 3, PTRB200_AF_GELU, 100, "rows_gemm_ws_fwd")
-            RW_CASE_K(RG_DGRAD, 3, PTRB200_AF_NONE, 100, "rows_gemm_ws_dgrad")
-            RW_CASE_K(RG_FWD, 1, PTRB200_AF_NONE, 136, "rows_gemm_ws_fwd") RW_CASE_K(RG_FWD, 1, PTRB200_AF_GELU, 100, "rows_gemm_ws_fwd")
-            RW_CASE_K(RG_DGRAD, 1, PTRB200_AF_NONE, 100, "rows_gemm_ws_dgrad")
-        }
+        // width-specialised instantiations for the default scorer (136 features, 100-wide hidden layers)
+        RW_CASE_K(RG_FWD, 3, PTRB200_AF_NONE, 136, "rows_gemm_ws_fwd") RW_CASE_K(RG_FWD, 3, PTRB200_AF_GELU, 100, "rows_gemm_ws_fwd")
+        RW_CASE_K(RG_DGRAD, 3, PTRB200_AF_NONE, 100, "rows_gemm_ws_dgrad")
+        RW_CASE_K(RG_FWD, 1, PTRB200_AF_NONE, 136, "rows_gemm_ws_fwd") RW_CASE_K(RG_FWD, 1, PTRB200_AF_GELU, 100, "rows_gemm_ws_fwd")
+        RW_CASE_K(RG_DGRAD, 1, PTRB200_AF_NONE, 100, "rows_gemm_ws_dgrad")
         RW_CASE(RG_FWD, 3, PTRB200_AF_NONE, "rows_gemm_ws_fwd") RW_CASE(RG_FWD, 3, PTRB200_AF_RELU, "rows_gemm_ws_fwd")
         RW_CASE(RG_FWD, 3, PTRB200_AF_GELU, "rows_gemm_ws_fwd") RW_CASE(RG_FWD, 3, PTRB200_AF_SIGM, "rows_gemm_ws_fwd")
         RW_CASE(RG_FWD, 3, -1, "rows_gemm_ws_fwd")
@@ -964,11 +935,12 @@ static void set_tiling(RowsGemmArgs& g, const Plan& p) {
     g.tile_rows = p.tile_rows; g.seg_len = p.seg_len; g.group_rows = p.group_rows; g.tiles_per_group = p.tiles_per_group;
 }
 
-// prologue that rebuilds the post-activation input of layer l from what layer l-1 stored
+// prologue that rebuilds the post-activation input of layer l from what layer l-1 stored (a ragged plan stores it whole)
 static void set_prologue(const ptrb200_ffnet* net, const Plan& p, int l, char* ws, const float* X,
                          const float*& P, const float*& scale, const float*& shift, int& act) {
     if (l == 0) { P = X; scale = shift = nullptr; act = PTRB200_AF_NONE; return; }
     const LayerPlan& prev = p.layer[l - 1];
+    if (p.ragged) { P = reinterpret_cast<const float*>(ws + prev.a_off); scale = shift = nullptr; act = PTRB200_AF_NONE; return; }
     P = reinterpret_cast<const float*>(ws + prev.z_off);
     scale = prev.has_norm ? reinterpret_cast<const float*>(ws + prev.scale_off) : nullptr;
     shift = prev.has_norm ? reinterpret_cast<const float*>(ws + prev.shift_off) : nullptr;
@@ -1067,179 +1039,96 @@ __global__ void __launch_bounds__(256) bn2_ragged_apply_kernel(const float* __re
     }
 }
 
-static int forward_ragged(const ptrb200_ffnet* net, const Plan& p, const float* X, const int32_t* offsets, float* out, char* ws,
-                          float drop, uint64_t seed, uint64_t offset, cudaStream_t st, bool fwd_only) {
-    int rc;
-    {   // operand images of every weight matrix (forward W, and W^T for the data gradients)
-        PackJobs jobs{};
-        int nj = 0, max_units = 0;
-        for (int l = 0; l < p.L; ++l) {
-            const LayerPlan& lp = p.layer[l];
-            for (int tr = 0; tr < (fwd_only ? 1 : 2); ++tr) {
-                if (tr == 1 && (l == 0 || lp.d_out % 4 != 0)) continue;
-                PackJob& j = jobs.job[nj++];
-                j.round_bf16 = p.bf16;
-                j.src = net->weight[l]; j.src_cols = lp.d_in; j.transpose = tr;
-                j.N = tr ? lp.d_in : lp.d_out; j.K = tr ? lp.d_out : lp.d_in;
-                j.NP = ((j.N + 15) / 16) * 16; j.nchunks = (j.K + 31) / 32;
-                j.img_hi = reinterpret_cast<unsigned char*>(ws + (tr ? lp.img_d_hi : lp.img_f_hi));
-                j.img_lo = p.passes == 3 ? reinterpret_cast<unsigned char*>(ws + (tr ? lp.img_d_lo : lp.img_f_lo)) : nullptr;
-                const int units = j.nchunks * j.NP * 8;
-                max_units = units > max_units ? units : max_units;
-            }
-        }
-        PTRB200_LAUNCH(pack_b_images_kernel, dim3((max_units + 255) / 256, nj), 256, 0, st, jobs);
-    }
-    const float* in = X;
+// operand images of every weight matrix (and, for the backward pass, of its transpose) in one launch
+static void pack_weight_images(const ptrb200_ffnet* net, const Plan& p, char* ws, bool fwd_only, cudaStream_t st) {
+    PackJobs jobs{};
+    int nj = 0, max_units = 0;
     for (int l = 0; l < p.L; ++l) {
         const LayerPlan& lp = p.layer[l];
-        const bool last = l == p.L - 1;
-        const bool bare = !lp.has_act && !lp.has_norm;
-        float* Z = (last && bare) ? out : reinterpret_cast<float*>(ws + lp.z_off);
+        for (int tr = 0; tr < (fwd_only ? 1 : 2); ++tr) {
+            if (tr == 1 && (l == 0 || lp.d_out % 4 != 0)) continue;     // dgrad images: only where launch_dgrad runs the tensor-core dgrad
+            PackJob& j = jobs.job[nj++];
+            j.round_bf16 = p.bf16;
+            j.src = net->weight[l]; j.src_cols = lp.d_in; j.transpose = tr;
+            j.N = tr ? lp.d_in : lp.d_out; j.K = tr ? lp.d_out : lp.d_in;
+            j.NP = ((j.N + 15) / 16) * 16; j.nchunks = (j.K + 31) / 32;
+            j.img_hi = reinterpret_cast<unsigned char*>(ws + (tr ? lp.img_d_hi : lp.img_f_hi));
+            j.img_lo = p.passes == 3 ? reinterpret_cast<unsigned char*>(ws + (tr ? lp.img_d_lo : lp.img_f_lo)) : nullptr;
+            const int units = j.nchunks * j.NP * 8;
+            max_units = units > max_units ? units : max_units;
+        }
+    }
+    PTRB200_LAUNCH(pack_b_images_kernel, dim3((max_units + 255) / 256, nj), 256, 0, st, jobs);
+}
+
+// dW[N,K] = sum_rows dZ^T (x) P on tensor cores.  The caller fills the operands of w (dZ, P, dropout, partials, rows and,
+// for the folded normalisation backward, Z2 and the coefficients); grid.x persistent CTAs per (dZ block, input block)
+// each write one partial, which reduce_splits_kernel sums in a fixed order.
+static int launch_wgrad(WgradArgs& w, int N, int K, int kb, dim3 grid, int passes, float* dW, cudaStream_t st) {
+    int rc;
+    const bool fused_dz = w.Z2 != nullptr;
+    w.N_full = N; w.K_full = K; w.kb = kb;
+    w.N = N < 128 ? N : 128; w.K = kb;       // block maxima (buffer geometry)
+    w.KP = ((w.K + 15) / 16) * 16;
+    const size_t smem = wgrad_smem(w.N, w.K, w.KP, w.tile_rows, passes, w.stages, fused_dz, fused_dz ? 24 : 8);
+    if (passes == 3) { if ((rc = opt_in_smem(wgrad_tc_kernel<3>, smem))) return rc; PTRB200_LAUNCH_TAG("wgrad_tc", wgrad_tc_kernel<3>, grid, WG_THREADS, smem, st, w); }
+    else { if ((rc = opt_in_smem(wgrad_tc_kernel<1>, smem))) return rc; PTRB200_LAUNCH_TAG("wgrad_tc", wgrad_tc_kernel<1>, grid, WG_THREADS, smem, st, w); }
+    PTRB200_LAUNCH(reduce_splits_kernel, (N * K + 63) / 64, 256, 0, st, (const float*)w.partials, dW, (int)grid.x, N * K);
+    return PTRB200_OK;
+}
+
+// dIn = dropmask(dZ W) of layer l: the tensor-core dgrad when d_out % 4 == 0, the outer product when the layer has a single
+// output, else the SIMT GEMM.  Z non-NULL (tensor-core dgrad only): dZ holds dY and the normalisation backward
+// k1*dY + k3*Z + k0 is folded into the operand staging, with the coefficients dy_finalize_kernel left in the workspace.
+static int launch_dgrad(const ptrb200_ffnet* net, const Plan& p, int l, char* ws, const float* dZ, const float* Z, float* dIn,
+                        DropCfg drop, cudaStream_t st) {
+    const LayerPlan& lp = p.layer[l];
+    if (lp.d_out % 4 == 0) {
+        const int NPl = ((lp.d_in + 15) / 16) * 16, nch = (lp.d_out + 31) / 32;
+        unsigned char* ih = reinterpret_cast<unsigned char*>(ws + lp.img_d_hi);
+        unsigned char* il = p.passes == 3 ? reinterpret_cast<unsigned char*>(ws + lp.img_d_lo) : nullptr;
+        if (l == 0)     // (layer 0's transpose image is only needed when dX is requested; deeper layers were packed by the forward call)
+            PTRB200_LAUNCH(pack_b_image_kernel<true>, (nch * NPl * 8 + 255) / 256, 256, 0, st, net->weight[l], lp.d_out, lp.d_in, ih, il, lp.d_in, NPl, lp.d_out, nch, (int)p.bf16);
         RowsGemmArgs g{};
         g.round_bf16 = p.bf16;
-        g.P = in; g.scale = g.shift = nullptr; g.act = PTRB200_AF_NONE; g.gr_prev = (int)p.rows;
-        g.drop = make_drop(last ? 0.0f : drop, seed, offset * 64 + (uint64_t)l);
-        g.bias = net->bias[l]; g.Out = Z;
-        g.a_out = (l > 0 && !fwd_only) ? reinterpret_cast<float*>(ws + lp.ain_off) : nullptr;     // dropout(A_{l-1}) for the weight gradient
-        g.partials = nullptr;
-        g.rows = (int)p.rows; g.K = lp.d_in; g.N = lp.d_out;
-        g.b_img_hi = reinterpret_cast<unsigned char*>(ws + lp.img_f_hi);
-        g.b_img_lo = p.passes == 3 ? reinterpret_cast<unsigned char*>(ws + lp.img_f_lo) : nullptr;
+        g.P = dZ; g.scale = g.shift = nullptr; g.act = PTRB200_AF_NONE; g.gr_prev = (int)p.rows;
+        if (Z) {
+            g.P2 = Z; g.gr_cur = p.gr;
+            g.kc1 = reinterpret_cast<const float*>(ws + p.k1_off); g.kc3 = reinterpret_cast<const float*>(ws + p.k3_off); g.kc0 = reinterpret_cast<const float*>(ws + p.k0_off);
+        }
+        g.drop = drop;
+        g.b_img_hi = ih; g.b_img_lo = il; g.bias = nullptr; g.Out = dIn; g.partials = nullptr;
+        g.rows = (int)p.rows; g.K = lp.d_out; g.N = lp.d_in;
         g.tile_rows = 128; g.seg_len = 128; g.group_rows = 0; g.tiles_per_group = 0;
-        if ((rc = launch_rows_gemm(RG_FWD, p.passes, g, p.ntiles, st, 0, nullptr, 1))) return rc;
-        if (bare) { in = Z; continue; }
-        NormRef nr = norm_ref(net, p, l, ws);
-        if (lp.has_norm)
-            PTRB200_LAUNCH(bn2_ragged_moments_kernel, p.G, dim3(32, 8), 0, st, (const float*)Z, offsets,
-                           reinterpret_cast<float*>(ws + lp.mean_off), reinterpret_cast<float*>(ws + lp.rstd_off), lp.d_out);
-        float* A = last ? out : reinterpret_cast<float*>(ws + lp.a_off);
-        if (lp.has_norm) PTRB200_LAUNCH(bn2_ragged_act_kernel, p.G, dim3(32, 8), 0, st, (const float*)Z, A, nr, offsets, lp.d_out);
-        else { const size_t total = p.rows * lp.d_out; PTRB200_LAUNCH(norm_act_fwd_kernel, elementwise_blocks(total), 256, 0, st, (const float*)Z, A, nr, total, lp.d_out, (int)p.rows); }
-        in = A;
+        return launch_rows_gemm(RG_DGRAD, p.passes, g, (int)((p.rows + 127) / 128), st);
     }
-    return check_launch("ffnet_forward(ragged)");
+    if (lp.d_out == 1 && lp.d_in % 4 == 0) {
+        const size_t units = p.rows * (lp.d_in / 4);
+        PTRB200_LAUNCH(dgrad_rank1_kernel, elementwise_blocks(units), 256, 0, st, dZ, net->weight[l], dIn, units, lp.d_in, drop, (int)p.bf16);
+        return PTRB200_OK;
+    }
+    GemmArgs g{};
+    g.A = dZ; g.Bm = net->weight[l]; g.C = dIn;
+    g.rows = (int)p.rows; g.d_in = lp.d_in; g.d_out = lp.d_out;
+    g.M = (int)p.rows; g.N = lp.d_in; g.K = lp.d_out;
+    g.drop = drop;
+    launch_gemm<GEMM_BWD_DATA>(g, 1, st);
+    return PTRB200_OK;
 }
 
-static int backward_ragged(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, const Plan& p, const float* X, const int32_t* offsets,
-                           const float* dOut, float* dX, char* ws, float drop, uint64_t seed, uint64_t offset, cudaStream_t st) {
-    int rc;
-    double* part = reinterpret_cast<double*>(ws + p.partials_off);
-    float* S1 = reinterpret_cast<float*>(ws + p.s1_off);
-    float* S2 = reinterpret_cast<float*>(ws + p.s2_off);
-    float* dbuf[2] = {reinterpret_cast<float*>(ws + p.dbuf0_off), reinterpret_cast<float*>(ws + p.dbuf1_off)};
-    float* wpart = reinterpret_cast<float*>(ws + p.wpart_off);
-    const float* dA = dOut;
-    int flip = 0;
-    for (int l = p.L - 1; l >= 0; --l) {
-        const LayerPlan& lp = p.layer[l];
-        const bool last = l == p.L - 1;
-        if (!grads->weight[l] || !grads->bias[l]) { set_error("ffnet_backward: layer %d grad buffers NULL", l); return PTRB200_ERR_INVALID; }
-        const float* Z = reinterpret_cast<const float*>(ws + lp.z_off);
-        const float* dZ = dA;
-        NormRef nr = norm_ref(net, p, l, ws);
-        if (lp.has_norm) {
-            float* dY = dbuf[flip]; flip ^= 1;
-            PTRB200_LAUNCH(bn2_ragged_dy_kernel, p.G, dim3(32, 8), 0, st, Z, dA, dY, nr, offsets, part, lp.d_out);
-            DyTail tail{};
-            tail.nr = nr; tail.gr = 1;
-            tail.bias_grad = grads->bias[l]; tail.bias_mode = 1;
-            tail.dgamma = grads->gamma[l]; tail.dbeta = grads->beta[l];
-            if (net->norm_affine) { tail.daff_w = grads->aff_w[l]; tail.daff_b = grads->aff_b[l]; }
-            PTRB200_LAUNCH(dy_finalize_kernel, lp.d_out, FIN_THREADS, 0, st, (const double*)part, S1, S2, (float*)nullptr, (float*)nullptr, p.G, lp.d_out, 1, tail);
-            PTRB200_LAUNCH(bn2_ragged_apply_kernel, p.G, dim3(32, 8), 0, st, Z, dY, nr, (const float*)S1, (const float*)S2, offsets, lp.d_out);
-            dZ = dY;
-        } else if (lp.has_act) {          // activation without a norm (not produced by get_stacked_FFNet with BN2, kept for completeness)
-            float* dY = dbuf[flip]; flip ^= 1;
-            launch_colstat<STAT_DY>(st, "colstat_dy", Z, dA, dY, nr, part, 1, 1, (int)p.rows, lp.d_out, (int)p.rows);
-            DyTail tail{};
-            tail.nr = nr; tail.gr = (int)p.rows; tail.bias_grad = grads->bias[l]; tail.bias_mode = 2;
-            PTRB200_LAUNCH(dy_finalize_kernel, lp.d_out, FIN_THREADS, 0, st, (const double*)part, (float*)nullptr, (float*)nullptr, (float*)nullptr, (float*)nullptr, 1, lp.d_out, 1, tail);
-            dZ = dY;
-        } else {                          // bare Linear: the bias gradient is the column sum of the incoming gradient
-            launch_colstat<STAT_COLSUM>(st, "colstat_colsum", dA, nullptr, nullptr, nr, part, 1, 1, (int)p.rows, lp.d_out, (int)p.rows);
-            PTRB200_LAUNCH(dy_finalize_kernel, lp.d_out, FIN_THREADS, 0, st, (const double*)part, (float*)nullptr, (float*)nullptr, grads->bias[l], (float*)nullptr, 1, lp.d_out, 1, DyTail{});
-        }
-        const float layer_drop = last ? 0.0f : drop;
-        {   // dW = sum_rows dZ^T (x) dropout(layer input)
-            WgradArgs w{};
-            w.round_bf16 = p.bf16;
-            w.dZ = dZ;
-            w.scale = w.shift = nullptr; w.act = PTRB200_AF_NONE; w.gr_prev = (int)p.rows;
-            if (l == 0) { w.P = X; w.drop = make_drop(layer_drop, seed, offset * 64 + (uint64_t)l); }
-            else { w.P = reinterpret_cast<const float*>(ws + lp.ain_off); w.drop = make_drop(0.0f, 0, 0); }
-            w.partials = wpart;
-            const WgBlocks wb = wgrad_blocks(lp.d_out, lp.d_in);
-            w.rows = (int)p.rows; w.N_full = lp.d_out; w.K_full = lp.d_in; w.kb = wb.kb;
-            w.N = lp.d_out < 128 ? lp.d_out : 128; w.K = wb.kb;
-            w.KP = ((w.K + 15) / 16) * 16;
-            w.tile_rows = p.wg_rows;
-            const size_t smem = wgrad_smem(w.N, w.K, w.KP, w.tile_rows, p.passes, w.stages, false, 8);
-            const dim3 grid(wb.gx, wb.mblocks, wb.kblocks);
-            if (p.passes == 3) { if ((rc = opt_in_smem(wgrad_tc_kernel<3>, smem))) return rc; PTRB200_LAUNCH_TAG("wgrad_tc", wgrad_tc_kernel<3>, grid, WG_THREADS, smem, st, w); }
-            else { if ((rc = opt_in_smem(wgrad_tc_kernel<1>, smem))) return rc; PTRB200_LAUNCH_TAG("wgrad_tc", wgrad_tc_kernel<1>, grid, WG_THREADS, smem, st, w); }
-            const int cnt = lp.d_in * lp.d_out;
-            PTRB200_LAUNCH(reduce_splits_kernel, (cnt + 63) / 64, 256, 0, st, (const float*)wpart, grads->weight[l], wb.gx, cnt);
-            if ((rc = call_hook(PTRB200_HOOK_LAYER_GRADS_READY, l, nullptr, 0, st))) return rc;
-        }
-        if (l > 0 || dX) {   // dIn = dropmask(dZ W)
-            float* dIn = l == 0 ? dX : dbuf[flip];
-            if (l > 0) flip ^= 1;
-            if (lp.d_out % 4 == 0) {
-                const int NPl = ((lp.d_in + 15) / 16) * 16, nch = (lp.d_out + 31) / 32;
-                unsigned char* ih = reinterpret_cast<unsigned char*>(ws + lp.img_d_hi);
-                unsigned char* il = p.passes == 3 ? reinterpret_cast<unsigned char*>(ws + lp.img_d_lo) : nullptr;
-                if (l == 0)
-                    PTRB200_LAUNCH(pack_b_image_kernel<true>, (nch * NPl * 8 + 255) / 256, 256, 0, st, net->weight[l], lp.d_out, lp.d_in, ih, il, lp.d_in, NPl, lp.d_out, nch, (int)p.bf16);
-                RowsGemmArgs g{};
-                g.round_bf16 = p.bf16;
-                g.P = dZ; g.scale = g.shift = nullptr; g.act = PTRB200_AF_NONE; g.gr_prev = (int)p.rows;
-                g.drop = make_drop(layer_drop, seed, offset * 64 + (uint64_t)l);
-                g.b_img_hi = ih; g.b_img_lo = il; g.bias = nullptr; g.Out = dIn; g.partials = nullptr;
-                g.rows = (int)p.rows; g.K = lp.d_out; g.N = lp.d_in;
-                g.tile_rows = 128; g.seg_len = 128; g.group_rows = 0; g.tiles_per_group = 0;
-                if ((rc = launch_rows_gemm(RG_DGRAD, p.passes, g, (int)((p.rows + 127) / 128), st, 0, nullptr, 1))) return rc;
-            } else if (lp.d_out == 1 && lp.d_in % 4 == 0) {
-                const size_t units = p.rows * (lp.d_in / 4);
-                PTRB200_LAUNCH(dgrad_rank1_kernel, elementwise_blocks(units), 256, 0, st, dZ, net->weight[l], dIn, units, lp.d_in,
-                               make_drop(layer_drop, seed, offset * 64 + (uint64_t)l), (int)p.bf16);
-            } else {
-                GemmArgs g{};
-                g.A = dZ; g.Bm = net->weight[l]; g.C = dIn;
-                g.rows = (int)p.rows; g.d_in = lp.d_in; g.d_out = lp.d_out;
-                g.M = (int)p.rows; g.N = lp.d_in; g.K = lp.d_out;
-                g.drop = make_drop(layer_drop, seed, offset * 64 + (uint64_t)l);
-                launch_gemm<GEMM_BWD_DATA>(g, 1, st);
-            }
-            dA = dIn;
-        }
-    }
-    return check_launch("ffnet_backward(ragged)");
+// norm-parameter gradient buffers of layer l (BN: gamma/beta only when affine; BN2: gamma/beta, and aff_w/aff_b when affine)
+static void set_norm_grads(DyTail& t, const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, int l) {
+    if (net->norm == PTRB200_NORM_BN) { if (net->norm_affine) { t.dgamma = grads->gamma[l]; t.dbeta = grads->beta[l]; } }
+    else { t.dgamma = grads->gamma[l]; t.dbeta = grads->beta[l]; if (net->norm_affine) { t.daff_w = grads->aff_w[l]; t.daff_b = grads->aff_b[l]; } }
 }
 
-static int forward_tc(const ptrb200_ffnet* net, const Plan& p, const float* X, float* out, char* ws,
+// Dense and ragged plans share the contractions; p.ragged (per-query BN2 over a ragged batch) only changes the
+// normalisation step: per-query bn2_ragged_* kernels on a materialised layer input instead of the epilogue statistics
+// partials and the normalisation folded into the next layer's prologue.
+static int forward_tc(const ptrb200_ffnet* net, const Plan& p, const float* X, const int32_t* offsets, float* out, char* ws,
                       float drop, uint64_t seed, uint64_t offset, cudaStream_t st, bool fwd_only) {
     int rc;
-    {   // operand images of every weight matrix (and, for the backward pass, of its transpose) in one launch
-        PackJobs jobs{};
-        int nj = 0, max_units = 0;
-        for (int l = 0; l < p.L; ++l) {
-            const LayerPlan& lp = p.layer[l];
-            for (int tr = 0; tr < (fwd_only ? 1 : 2); ++tr) {
-                if (tr == 1 && (l == 0 || lp.d_out % 4 != 0)) continue;     // dgrad images: only where backward_tc runs the tensor-core dgrad
-                PackJob& j = jobs.job[nj++];
-                j.round_bf16 = p.bf16;
-                j.src = net->weight[l]; j.src_cols = lp.d_in; j.transpose = tr;
-                j.N = tr ? lp.d_in : lp.d_out; j.K = tr ? lp.d_out : lp.d_in;
-                j.NP = ((j.N + 15) / 16) * 16; j.nchunks = (j.K + 31) / 32;
-                j.img_hi = reinterpret_cast<unsigned char*>(ws + (tr ? lp.img_d_hi : lp.img_f_hi));
-                j.img_lo = p.passes == 3 ? reinterpret_cast<unsigned char*>(ws + (tr ? lp.img_d_lo : lp.img_f_lo)) : nullptr;
-                const int units = j.nchunks * j.NP * 8;
-                max_units = units > max_units ? units : max_units;
-            }
-        }
-        PTRB200_LAUNCH(pack_b_images_kernel, dim3((max_units + 255) / 256, nj), 256, 0, st, jobs);
-    }
+    pack_weight_images(net, p, ws, fwd_only, st);
     for (int l = 0; l < p.L; ++l) {
         const LayerPlan& lp = p.layer[l];
         const bool last = l == p.L - 1;
@@ -1251,15 +1140,24 @@ static int forward_tc(const ptrb200_ffnet* net, const Plan& p, const float* X, f
         g.drop = make_drop(last ? 0.0f : drop, seed, offset * 64 + (uint64_t)l);
         g.bias = net->bias[l]; g.Out = Z;
         g.a_out = (l > 0 && !fwd_only) ? reinterpret_cast<float*>(ws + lp.ain_off) : nullptr;     // a by-product for the backward pass
-        g.partials = lp.has_norm ? reinterpret_cast<double*>(ws + p.partials_off) : nullptr;
+        g.partials = (lp.has_norm && !p.ragged) ? reinterpret_cast<double*>(ws + p.partials_off) : nullptr;
         g.rows = (int)p.rows; g.K = lp.d_in; g.N = lp.d_out;
         g.b_img_hi = reinterpret_cast<unsigned char*>(ws + lp.img_f_hi);
         g.b_img_lo = p.passes == 3 ? reinterpret_cast<unsigned char*>(ws + lp.img_f_lo) : nullptr;
         set_tiling(g, p);
         int S_fwd = p.S_stat;
-        const int stats_kind = !lp.has_norm ? 0 : (net->norm == PTRB200_NORM_BN ? 1 : 2);
+        const int stats_kind = !g.partials ? 0 : (net->norm == PTRB200_NORM_BN ? 1 : 2);
         if ((rc = launch_rows_gemm(RG_FWD, p.passes, g, p.ntiles, st, stats_kind, &S_fwd, p.S_stat))) return rc;
         NormRef nr = norm_ref(net, p, l, ws);
+        if (p.ragged) {
+            if (lp.has_norm) {      // (under BN2 every layer with an activation has a norm)
+                float* A = last ? out : reinterpret_cast<float*>(ws + lp.a_off);
+                PTRB200_LAUNCH(bn2_ragged_moments_kernel, p.G, dim3(32, 8), 0, st, (const float*)Z, offsets,
+                               reinterpret_cast<float*>(ws + lp.mean_off), reinterpret_cast<float*>(ws + lp.rstd_off), lp.d_out);
+                PTRB200_LAUNCH(bn2_ragged_act_kernel, p.G, dim3(32, 8), 0, st, (const float*)Z, A, nr, offsets, lp.d_out);
+            }
+            continue;
+        }
         if (lp.has_norm) {
             const int cnt = p.G * lp.d_out;
             const double* part = g.partials;
@@ -1283,7 +1181,7 @@ static int forward_tc(const ptrb200_ffnet* net, const Plan& p, const float* X, f
     return check_launch("ffnet_forward(tc)");
 }
 
-static int backward_tc(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, const Plan& p, const float* X,
+static int backward_tc(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, const Plan& p, const float* X, const int32_t* offsets,
                        const float* dOut, float* dX, char* ws, float drop, uint64_t seed, uint64_t offset, cudaStream_t st) {
     int rc;
     double* part = reinterpret_cast<double*>(ws + p.partials_off);
@@ -1303,13 +1201,10 @@ static int backward_tc(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grad
         bool fuse_dz = false;
         NormRef nr = norm_ref(net, p, l, ws);
         const size_t total = p.rows * lp.d_out;
-        dim3 sgrid(p.G, p.S_stat);
-        // the backward statistics pass picks its own slicing: long slices amortise the per-CTA reduction
-        int bS = p.S_stat, bslice = p.slice_rows;
-        // (128-row slices, equal to the forward tiling)
         if (lp.has_act || lp.has_norm) {
             float* dY = dbuf[flip]; flip ^= 1;
-            launch_colstat<STAT_DY>(st, "colstat_dy", Z, dA, dY, nr, part, p.G, bS, p.gr, lp.d_out, bslice, r1);
+            if (p.ragged) PTRB200_LAUNCH(bn2_ragged_dy_kernel, p.G, dim3(32, 8), 0, st, Z, dA, dY, nr, offsets, part, lp.d_out);
+            else launch_colstat<STAT_DY>(st, "colstat_dy", Z, dA, dY, nr, part, p.G, p.S_stat, p.gr, lp.d_out, p.slice_rows, r1);
             r1.w = nullptr;
             // one finalize launch: channel sums -> norm-parameter gradients, bias gradient, folded-dZ coefficients
             DyTail tail{};
@@ -1319,16 +1214,16 @@ static int backward_tc(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grad
             // per-channel shift); the reference's autograd produces rounding noise there.
             tail.bias_mode = lp.has_norm ? 1 : 2;
             if (lp.has_norm) {
-                if (net->norm == PTRB200_NORM_BN) { if (net->norm_affine) { tail.dgamma = grads->gamma[l]; tail.dbeta = grads->beta[l]; } }
-                else { tail.dgamma = grads->gamma[l]; tail.dbeta = grads->beta[l]; if (net->norm_affine) { tail.daff_w = grads->aff_w[l]; tail.daff_b = grads->aff_b[l]; } }
+                set_norm_grads(tail, net, grads, l);
                 // fold dZ = a*rstd*(dY - S1/N - xhat*S2/N) into the operand staging of dgrad and wgrad when both can take it
                 // (saves one 12-bytes-per-element pass); otherwise materialise dZ in place
                 int Rf = 32, stf = 0;
                 const int KPl = ((lp.d_in + 15) / 16) * 16;
-                fuse_dz = lp.d_out % 4 == 0 && lp.d_out <= 128 && lp.d_in <= 256 && (l == 0 || rows_ws_fits(lp.d_out, lp.d_in, p.passes)) &&
+                fuse_dz = !p.ragged && lp.d_out % 4 == 0 && lp.d_out <= 128 && lp.d_in <= 256 && (l == 0 || rows_ws_fits(lp.d_out, lp.d_in, p.passes)) &&
                           wgrad_smem(lp.d_out, lp.d_in, KPl, Rf, p.passes, stf, true, 24) <= (size_t)227 * 1024;
                 if (fuse_dz) { tail.k1 = reinterpret_cast<float*>(ws + p.k1_off); tail.k3 = reinterpret_cast<float*>(ws + p.k3_off); tail.k0 = reinterpret_cast<float*>(ws + p.k0_off); }
             }
+            int bS = p.S_stat;
             const double* fin_part = part;
             const double* gcount = nullptr;
             if (lp.has_norm && p.sync_bn) {   // S1 = sum dY, S2 = sum dY*xhat over the GLOBAL batch (same exchange as the forward moments)
@@ -1341,92 +1236,50 @@ static int backward_tc(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grad
             PTRB200_LAUNCH(dy_finalize_kernel, lp.d_out, FIN_THREADS, 0, st, fin_part,
                            (lp.has_norm && !fuse_dz) ? S1 : (float*)nullptr, (lp.has_norm && !fuse_dz) ? S2 : (float*)nullptr,
                            (float*)nullptr, (float*)nullptr, p.G, lp.d_out, bS, tail);
-            if (lp.has_norm) {
-                if (fuse_dz) {
-                } else if (lp.d_out % 4 == 0) PTRB200_LAUNCH(norm_bwd_apply4_kernel, elementwise_blocks(total / 4), 256, 0, st, Z, dY, nr, (const float*)S1, (const float*)S2, total / 4, lp.d_out, p.gr, gcount);
+            if (lp.has_norm && !fuse_dz) {
+                if (p.ragged) PTRB200_LAUNCH(bn2_ragged_apply_kernel, p.G, dim3(32, 8), 0, st, Z, dY, nr, (const float*)S1, (const float*)S2, offsets, lp.d_out);
+                else if (lp.d_out % 4 == 0) PTRB200_LAUNCH(norm_bwd_apply4_kernel, elementwise_blocks(total / 4), 256, 0, st, Z, dY, nr, (const float*)S1, (const float*)S2, total / 4, lp.d_out, p.gr, gcount);
                 else PTRB200_LAUNCH(norm_bwd_apply_kernel, elementwise_blocks(total), 256, 0, st, Z, dY, nr, (const float*)S1, (const float*)S2, total, lp.d_out, p.gr, gcount);
             }
             dZ = dY;
-        } else {
-            launch_colstat<STAT_COLSUM>(st, "colstat_colsum", dA, nullptr, nullptr, nr, part, p.G, p.S_stat, p.gr, lp.d_out, p.slice_rows);
-            PTRB200_LAUNCH(dy_finalize_kernel, lp.d_out, FIN_THREADS, 0, st, (const double*)part, (float*)nullptr, (float*)nullptr, grads->bias[l], (float*)nullptr, p.G, lp.d_out, p.S_stat, DyTail{});
+        } else {        // bare Linear: the bias gradient is the column sum of the incoming gradient (a ragged batch: one group)
+            const int G = p.ragged ? 1 : p.G, gr = p.ragged ? (int)p.rows : p.gr;
+            launch_colstat<STAT_COLSUM>(st, "colstat_colsum", dA, nullptr, nullptr, nr, part, G, p.S_stat, gr, lp.d_out, p.slice_rows);
+            PTRB200_LAUNCH(dy_finalize_kernel, lp.d_out, FIN_THREADS, 0, st, (const double*)part, (float*)nullptr, (float*)nullptr, grads->bias[l], (float*)nullptr, G, lp.d_out, p.S_stat, DyTail{});
         }
-        const float layer_drop = last ? 0.0f : drop;
-        // ---- dW on tensor cores: sum_rows dZ^T (x) rebuilt layer input ----
-        {
+        const DropCfg layer_drop = make_drop(last ? 0.0f : drop, seed, offset * 64 + (uint64_t)l);
+        {   // dW = sum_rows dZ^T (x) layer input: dropout(X) rebuilt on the fly for layer 0, the operand the forward kernel built for deeper layers
             WgradArgs w{};
             w.round_bf16 = p.bf16;
             w.dZ = dZ;
-            if (l == 0) {          // layer 0 input = dropout(X): rebuilt on the fly
-                w.P = X; w.scale = w.shift = nullptr; w.act = PTRB200_AF_NONE;
-                w.drop = make_drop(layer_drop, seed, offset * 64 + (uint64_t)l);
-            } else {               // deeper layers read the operand the forward kernel already built
-                w.P = reinterpret_cast<const float*>(ws + lp.ain_off); w.scale = w.shift = nullptr; w.act = PTRB200_AF_NONE;
-                w.drop = make_drop(0.0f, 0, 0);
-            }
-            w.gr_prev = p.gr;
+            if (l == 0) { w.P = X; w.drop = layer_drop; }
+            else { w.P = reinterpret_cast<const float*>(ws + lp.ain_off); w.drop = make_drop(0.0f, 0, 0); }
             w.partials = wpart;
-            const WgBlocks wb = wgrad_blocks(lp.d_out, lp.d_in);
-            w.rows = (int)p.rows; w.N_full = lp.d_out; w.K_full = lp.d_in; w.kb = wb.kb;
-            w.N = lp.d_out < 128 ? lp.d_out : 128; w.K = wb.kb;       // block maxima (buffer geometry)
-            w.KP = ((w.K + 15) / 16) * 16;
-            w.tile_rows = p.wg_rows;
+            w.rows = (int)p.rows;
             if (fuse_dz) {
                 w.Z2 = Z; w.gr_cur = p.gr;
                 w.kc1 = reinterpret_cast<const float*>(ws + p.k1_off); w.kc3 = reinterpret_cast<const float*>(ws + p.k3_off); w.kc0 = reinterpret_cast<const float*>(ws + p.k0_off);
             }
-            const size_t smem = wgrad_smem(w.N, w.K, w.KP, w.tile_rows, p.passes, w.stages, fuse_dz, fuse_dz ? 24 : 8);
-            const dim3 grid(wb.gx, wb.mblocks, wb.kblocks);   // persistent CTAs per (dZ block, input block), fed by the TMA ring
-            if (p.passes == 3) { if ((rc = opt_in_smem(wgrad_tc_kernel<3>, smem))) return rc; PTRB200_LAUNCH_TAG("wgrad_tc", wgrad_tc_kernel<3>, grid, WG_THREADS, smem, st, w); }
-            else { if ((rc = opt_in_smem(wgrad_tc_kernel<1>, smem))) return rc; PTRB200_LAUNCH_TAG("wgrad_tc", wgrad_tc_kernel<1>, grid, WG_THREADS, smem, st, w); }
-            const int cnt = lp.d_in * lp.d_out;
-            PTRB200_LAUNCH(reduce_splits_kernel, (cnt + 63) / 64, 256, 0, st, (const float*)wpart, grads->weight[l], wb.gx, cnt);
+            const WgBlocks wb = wgrad_blocks(lp.d_out, lp.d_in);
+            if ((rc = launch_wgrad(w, lp.d_out, lp.d_in, wb.kb, dim3(wb.gx, wb.mblocks, wb.kblocks), p.passes, grads->weight[l], st))) return rc;
             // every parameter gradient of layer l is now enqueued: a data-parallel caller can start reducing it while the
             // layers below are still running (dist.GradBucket's overlapped all-reduce)
             if ((rc = call_hook(PTRB200_HOOK_LAYER_GRADS_READY, l, nullptr, 0, st))) return rc;
         }
-        // ---- dIn = dropmask(dZ * W) ----
         if (l > 0 || dX) {
             float* dIn = l == 0 ? dX : dbuf[flip];
             if (l > 0) flip ^= 1;
-            if (lp.d_out % 4 == 0) {
-                const int NPl = ((lp.d_in + 15) / 16) * 16, nch = (lp.d_out + 31) / 32;
-                unsigned char* ih = reinterpret_cast<unsigned char*>(ws + lp.img_d_hi);
-                unsigned char* il = p.passes == 3 ? reinterpret_cast<unsigned char*>(ws + lp.img_d_lo) : nullptr;
-                if (l == 0)     // (layer 0's transpose image is only needed when dX is requested; deeper layers were packed by the forward call)
-                    PTRB200_LAUNCH(pack_b_image_kernel<true>, (nch * NPl * 8 + 255) / 256, 256, 0, st, net->weight[l], lp.d_out, lp.d_in, ih, il, lp.d_in, NPl, lp.d_out, nch, (int)p.bf16);
-                RowsGemmArgs g{};
-                g.round_bf16 = p.bf16;
-                g.P = dZ; g.scale = g.shift = nullptr; g.act = PTRB200_AF_NONE; g.gr_prev = (int)p.rows;
-                if (fuse_dz) {
-                    g.P2 = Z; g.gr_cur = p.gr;
-                    g.kc1 = reinterpret_cast<const float*>(ws + p.k1_off); g.kc3 = reinterpret_cast<const float*>(ws + p.k3_off); g.kc0 = reinterpret_cast<const float*>(ws + p.k0_off);
-                }
-                g.drop = make_drop(layer_drop, seed, offset * 64 + (uint64_t)l);
-                g.b_img_hi = ih; g.b_img_lo = il; g.bias = nullptr; g.Out = dIn; g.partials = nullptr;
-                g.rows = (int)p.rows; g.K = lp.d_out; g.N = lp.d_in;
-                g.tile_rows = 128; g.seg_len = 128; g.group_rows = 0; g.tiles_per_group = 0;
-                if ((rc = launch_rows_gemm(RG_DGRAD, p.passes, g, (int)((p.rows + 127) / 128), st))) return rc;
-            } else if (lp.d_out == 1 && l > 0 && colstat_vectorised(lp.d_in) && (p.layer[l - 1].has_act || p.layer[l - 1].has_norm)) {
-                // the next iteration's statistics pass rebuilds dIn = dropmask(dz (x) w) on the fly
+            // the next iteration's statistics pass rebuilds dIn = dropmask(dz (x) w) on the fly (dense plans only: the
+            // per-query dY pass of a ragged batch reads a materialised dA)
+            if (!p.ragged && lp.d_out == 1 && l > 0 && colstat_vectorised(lp.d_in) && (p.layer[l - 1].has_act || p.layer[l - 1].has_norm)) {
                 r1.w = net->weight[l];
-                r1.drop = make_drop(layer_drop, seed, offset * 64 + (uint64_t)l);
+                r1.drop = layer_drop;
                 r1.round_bf16 = p.bf16;
                 flip ^= 1;                         // dIn's buffer stays unused; dZ (in the other one) must survive the next pass
                 dA = dZ;
                 continue;
-            } else if (lp.d_out == 1 && lp.d_in % 4 == 0) {
-                const size_t units = p.rows * (lp.d_in / 4);
-                PTRB200_LAUNCH(dgrad_rank1_kernel, elementwise_blocks(units), 256, 0, st, dZ, net->weight[l], dIn, units, lp.d_in,
-                               make_drop(layer_drop, seed, offset * 64 + (uint64_t)l), (int)p.bf16);
-            } else {
-                GemmArgs g{};
-                g.A = dZ; g.Bm = net->weight[l]; g.C = dIn;
-                g.rows = (int)p.rows; g.d_in = lp.d_in; g.d_out = lp.d_out;
-                g.M = (int)p.rows; g.N = lp.d_in; g.K = lp.d_out;
-                g.drop = make_drop(layer_drop, seed, offset * 64 + (uint64_t)l);
-                launch_gemm<GEMM_BWD_DATA>(g, 1, st);
             }
+            if ((rc = launch_dgrad(net, p, l, ws, dZ, fuse_dz ? Z : nullptr, dIn, layer_drop, st))) return rc;
             dA = dIn;
         }
     }
@@ -1450,18 +1303,11 @@ int ptrb200_tc_wgrad(const float* dZ, const float* P, float* dW, float* partials
     if (!dZ || !P || !dW || !partials || rows <= 0 || N <= 0 || K <= 0) { set_error("tc_wgrad: bad arguments"); return PTRB200_ERR_INVALID; }
     if (N > 128 || K > 256 || K % 4 != 0) { set_error("tc_wgrad: needs N <= 128, K <= 256, K %% 4 == 0"); return PTRB200_ERR_UNSUPPORTED; }
     WgradArgs w{};
-    w.dZ = dZ; w.P = P; w.scale = w.shift = nullptr; w.act = PTRB200_AF_NONE; w.gr_prev = rows;
+    w.dZ = dZ; w.P = P;
     w.drop = make_drop(0.0f, 0, 0); w.partials = partials;
-    w.rows = rows; w.K = K; w.N = N; w.KP = ((K + 15) / 16) * 16; w.tile_rows = 32;
-    w.N_full = N; w.K_full = K; w.kb = K;
-    const int grid = 296;
-    const size_t smem = wgrad_smem(N, K, w.KP, w.tile_rows, passes, w.stages);
-    int rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (passes == 3) { if ((rc = opt_in_smem(wgrad_tc_kernel<3>, smem))) return rc; PTRB200_LAUNCH_TAG("wgrad_tc", wgrad_tc_kernel<3>, grid, WG_THREADS, smem, st, w); }
-    else { if ((rc = opt_in_smem(wgrad_tc_kernel<1>, smem))) return rc; PTRB200_LAUNCH_TAG("wgrad_tc", wgrad_tc_kernel<1>, grid, WG_THREADS, smem, st, w); }
-    PTRB200_LAUNCH(reduce_splits_kernel, (N * K + 63) / 64, 256, 0, st, (const float*)partials, dW, grid, N * K);
-    return check_launch("tc_wgrad");
+    w.rows = rows;
+    const int rc = launch_wgrad(w, N, K, K, dim3(296), passes, dW, (cudaStream_t)stream);     // 296 partial slots (header)
+    return rc ? rc : check_launch("tc_wgrad");
 }
 
 int64_t ptrb200_ffnet_workspace_bytes(const ptrb200_ffnet* net, int B, int n, int total_rows) {
@@ -1491,8 +1337,7 @@ int ptrb200_ffnet_forward(const ptrb200_ffnet* net, const float* X, float* out, 
         padded = *net; padded.dims[0] = p.pad_k; padded.weight[0] = Wp;
         net = &padded; X = Xp;
     }
-    if (p.ragged) return forward_ragged(net, p, X, offsets, out, ws, drop, seed, offset, st, (training & PTRB200_FFNET_FORWARD_ONLY) != 0);
-    if (p.use_tc) return forward_tc(net, p, X, out, ws, drop, seed, offset, st, (training & PTRB200_FFNET_FORWARD_ONLY) != 0);
+    if (p.use_tc) return forward_tc(net, p, X, offsets, out, ws, drop, seed, offset, st, (training & PTRB200_FFNET_FORWARD_ONLY) != 0);
     const float* in = X;
     for (int l = 0; l < p.L; ++l) {
         const LayerPlan& lp = p.layer[l];
@@ -1546,22 +1391,17 @@ int ptrb200_ffnet_backward(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* 
         pg.weight[0] = reinterpret_cast<float*>(ws + p.dw0pad_off);
         float* dXp = dX ? reinterpret_cast<float*>(ws + p.dxpad_off) : nullptr;
         const float* Xp = reinterpret_cast<const float*>(ws + p.xpad_off);
-        rc = p.ragged ? backward_ragged(&padded, &pg, p, Xp, offsets, dOut, dXp, ws, drop, seed, offset, st)
-                      : backward_tc(&padded, &pg, p, Xp, dOut, dXp, ws, drop, seed, offset, st);
-        if (rc) return rc;
+        if ((rc = backward_tc(&padded, &pg, p, Xp, offsets, dOut, dXp, ws, drop, seed, offset, st))) return rc;
         if (!grads->weight[0]) { set_error("ffnet_backward: layer 0 grad buffer NULL"); return PTRB200_ERR_INVALID; }
         PTRB200_LAUNCH(copy_cols_kernel, elementwise_blocks((size_t)net->dims[1] * net->dims[0]), 256, 0, st, (const float*)pg.weight[0], grads->weight[0],
                        (size_t)net->dims[1], p.pad_k, net->dims[0]);
         if (dX) PTRB200_LAUNCH(copy_cols_kernel, elementwise_blocks(p.rows * net->dims[0]), 256, 0, st, (const float*)dXp, dX, p.rows, p.pad_k, net->dims[0]);
         return check_launch("ffnet_backward(padded)");
     }
-    if (p.ragged) return backward_ragged(net, grads, p, X, offsets, dOut, dX, ws, drop, seed, offset, st);
-    if (p.use_tc) return backward_tc(net, grads, p, X, dOut, dX, ws, drop, seed, offset, st);
+    if (p.use_tc) return backward_tc(net, grads, p, X, offsets, dOut, dX, ws, drop, seed, offset, st);
     double* part = reinterpret_cast<double*>(ws + p.partials_off);
     float* S1 = reinterpret_cast<float*>(ws + p.s1_off);
     float* S2 = reinterpret_cast<float*>(ws + p.s2_off);
-    float* T1 = reinterpret_cast<float*>(ws + p.t1_off);
-    float* T2 = reinterpret_cast<float*>(ws + p.t2_off);
     float* dbuf[2] = {reinterpret_cast<float*>(ws + p.dbuf0_off), reinterpret_cast<float*>(ws + p.dbuf1_off)};
     float* wpart = reinterpret_cast<float*>(ws + p.wpart_off);
     const float* dA = dOut;                 // gradient w.r.t. the layer's post-activation output
@@ -1578,19 +1418,18 @@ int ptrb200_ffnet_backward(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* 
             float* dY = dbuf[flip]; flip ^= 1;
             dim3 grid(p.G, p.S_stat);
             PTRB200_LAUNCH(colstat_kernel<STAT_DY>, grid, dim3(32, 8), 0, st, Z, dA, dY, nr, part, p.gr, lp.d_out, p.S_stat, p.slice_rows);
+            // channel sums -> norm-parameter gradients, or without a norm the bias gradient (= sum dY)
+            DyTail tail{};
+            tail.nr = nr;
+            if (lp.has_norm) set_norm_grads(tail, net, grads, l);
+            else { tail.bias_grad = grads->bias[l]; tail.bias_mode = 2; }
             PTRB200_LAUNCH(dy_finalize_kernel, lp.d_out, FIN_THREADS, 0, st, (const double*)part,
-                           lp.has_norm ? S1 : (float*)nullptr, lp.has_norm ? S2 : (float*)nullptr, T1, T2, p.G, lp.d_out, p.S_stat, DyTail{});
+                           lp.has_norm ? S1 : (float*)nullptr, lp.has_norm ? S2 : (float*)nullptr, (float*)nullptr, (float*)nullptr, p.G, lp.d_out, p.S_stat, tail);
             if (lp.has_norm) {
-                float *dg = nullptr, *db = nullptr, *dw = nullptr, *dbw = nullptr;
-                if (net->norm == PTRB200_NORM_BN) { if (net->norm_affine) { dg = grads->gamma[l]; db = grads->beta[l]; } }
-                else { dg = grads->gamma[l]; db = grads->beta[l]; if (net->norm_affine) { dw = grads->aff_w[l]; dbw = grads->aff_b[l]; } }
-                PTRB200_LAUNCH(norm_param_grad_kernel, (lp.d_out + 127) / 128, 128, 0, st, nr, (const float*)T1, (const float*)T2, dg, db, dw, dbw, lp.d_out);
                 PTRB200_LAUNCH(norm_bwd_apply_kernel, elementwise_blocks(total), 256, 0, st, Z, dY, nr, (const float*)S1, (const float*)S2, total, lp.d_out, p.gr);
                 // bias gradient = column sums of dZ (zero up to rounding under a norm, as in the reference)
                 PTRB200_LAUNCH(colstat_kernel<STAT_COLSUM>, grid, dim3(32, 8), 0, st, (const float*)dY, (const float*)nullptr, (float*)nullptr, nr, part, p.gr, lp.d_out, p.S_stat, p.slice_rows);
                 PTRB200_LAUNCH(dy_finalize_kernel, lp.d_out, FIN_THREADS, 0, st, (const double*)part, (float*)nullptr, (float*)nullptr, grads->bias[l], (float*)nullptr, p.G, lp.d_out, p.S_stat, DyTail{});
-            } else {
-                cudaMemcpyAsync(grads->bias[l], T1, (size_t)lp.d_out * 4, cudaMemcpyDeviceToDevice, st);
             }
             dZ = dY;
         } else {

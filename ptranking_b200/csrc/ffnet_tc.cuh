@@ -48,7 +48,6 @@ struct RowsGemmArgs {
     int group_rows;        // BN2 with n > 128: rows per group (tiles restart at every group), else 0
     int tiles_per_group;
     int round_bf16;        // PTRB200_MATH_BF16: the A operand is rounded to bf16 on its way into shared memory
-    int no_partial;        // debugging switch (PTRB200_NO_PARTIAL=1): keep the regular unit mapping for a short last K-chunk
 };
 
 enum { RG_FWD = 0, RG_DGRAD = 1 };
@@ -555,7 +554,7 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
             const int lastc = nchunks - 1;
             const int vlast = (K - lastc * 32 + 3) >> 2;                // 16-byte units of the last chunk that hold data (1..8)
             // (forward only: the dgrad instantiation keeps the regular mapping, its fused staging already carries more live state)
-            const bool partial = MODE == RG_FWD && vlast < 8 && !g.no_partial;
+            const bool partial = MODE == RG_FWD && vlast < 8;
             const int zfill = 8;                                        // units the last chunk's MMAs read
             const int rB = ptid & 127;
             int jB_[RW_PU];

@@ -13,7 +13,6 @@
 //   ListMLE     ptranking/ltr_adhoc/listwise/listmle.py:83-97
 //   ApproxNDCG  ptranking/ltr_adhoc/listwise/approxNDCG.py:19-28,45-62
 //   nDCG@ks     ptranking/base/ranker.py:67-95, metric/adhoc/adhoc_metric.py:219-260
-#include <stdlib.h>
 #include "losses_common.cuh"
 
 namespace ptrb200 {
@@ -694,13 +693,12 @@ static int launch_pairwise(const float* scores, const float* labels, const int32
     if (rc) return rc;
     const int npow2 = next_pow2(n);
     const size_t smem = (LAMBDA ? (size_t)npow2 * 8 : 0) + (size_t)n * 4 * 6 + 33 * 4;
-    static const bool no_runs = getenv("PTRB200_NO_RUNS") != nullptr;      // debugging switch: keep the circulant schedule
     // tie pairs skipped: partners = the better-labelled prefix.  One thread per document up to 512; longer lists (up to 2048)
     // are walked in passes by 1024 threads (512 when the per-warp partner rows would not fit in shared memory otherwise)
     int threads = n <= 512 ? block_threads(n) : 1024;
     size_t smem_r = (size_t)npow2 * 8 + (size_t)n * 4 * 6 + 33 * 4 + (size_t)(threads / 32) * n * 4;
     if (smem_r > 227 * 1024 && n > 512) { threads = 512; smem_r = (size_t)npow2 * 8 + (size_t)n * 4 * 6 + 33 * 4 + (size_t)(threads / 32) * n * 4; }
-    if (LAMBDA && n <= 2048 && smem_r <= 227 * 1024 && !no_runs) {
+    if (LAMBDA && n <= 2048 && smem_r <= 227 * 1024) {
         if ((rc = allow_smem(lambdarank_runs_kernel, smem_r))) return rc;
         PTRB200_LAUNCH_TAG("pairwise_bce_kernel<LAMBDA>", lambdarank_runs_kernel, B, threads, smem_r, stream,
                            scores, labels, grad, loss_q, offsets, n, npow2, sigma);
