@@ -136,6 +136,22 @@ int ptrb200_softrank_fwd_bwd(const float* scores, const float* labels, const int
 int ptrb200_sinkstep(const float* dist, const float* log_nu, const float* log_u, float* log_v,
                      int B, int d1, int d2, float lambda, ptrb200_stream_t stream);
 
+/* WassRank.custom_loss_function in mode 'SinkhornOT' with 'ST'/'BothST' histograms,
+ * ptranking/ltr_adhoc/listwise/wassrank/wassRank.py:43-86, OldSinkhornOT at pytorch_wasserstein.py:323-394, costs of
+ * wasserstein_cost_mat.py:47-139.  Every query gets its own cost matrix (formed on the fly, never stored); the Sinkhorn
+ * iteration runs in the log domain.  loss_per_query[b] carries 1/batch_queries, so that their sum is the mean over the
+ * batch; grad is the reference's gradient: the dual potential lam*log_u, centred, divided by batch_queries, through the
+ * softmax of the scores.  batch_queries (>= B) is the query count of the whole batch: a length-bucket launch passes the
+ * full count.  sh_itr = 0 is legal. */
+#define PTRB200_WASS_COST_P1  0   /* |i - j|, positions 1..n */
+#define PTRB200_WASS_COST_P2  1   /* |i - j|^2 */
+#define PTRB200_WASS_COST_EG  2   /* explicit grouping: gain_base^y - 1 with the non-relevance gap, var_penalty within a label */
+#define PTRB200_WASS_COST_DG  3   /* |2^y_i - 2^y_j| */
+#define PTRB200_WASS_COST_DDG 4   /* dg times |1/log2(i+2) - 1/log2(j+2)|, 0-based positions */
+int ptrb200_wassrank_fwd_bwd(const float* scores, const float* labels, const int32_t* offsets, float* grad,
+                             float* loss_per_query, int B, int n, int batch_queries, int cost_type, float lam,
+                             int sh_itr, float non_rele_gap, float var_penalty, float gain_base, ptrb200_stream_t stream);
+
 /* deterministic (fixed-order) sum of n floats into out[0] -- the `torch.sum` over queries
  * that ends every reference loss (e.g. lambdarank.py:56). */
 int ptrb200_sum_f32(const float* x, float* out, int n, ptrb200_stream_t stream);

@@ -9,6 +9,7 @@ from __future__ import annotations
 import contextlib
 import ctypes as C
 import functools
+import math
 import os
 from typing import Optional, Sequence
 
@@ -96,6 +97,12 @@ def _loss_call(name: str, scores: torch.Tensor, labels: torch.Tensor, params: di
     # Length buckets pay for the O(n^2) losses only (the O(n) ones are launch-bound: one launch is best), and not for losses
     # coupled across the batch (ApproxNDCG's [B]/[B,1] broadcast, RankMSE's mean over queries)
     quadratic = name in ("RankNet", "LambdaRank", "LambdaLoss", "SoftRank", "ApproxNDCG")
+    if name == "WassRank":
+        cost = params.get("cost_type", "eg")
+        if cost not in _lib.WASS_COST_TYPES:
+            raise ValueError(f"WassRank cost_type must be one of {sorted(_lib.WASS_COST_TYPES)}, got {cost!r}")
+        # eg / dg take the kernel's O(n R) label-group schedule; the position-based costs walk all n^2 pairs
+        quadratic = cost in ("p1", "p2", "ddg")
     coupled = name == "RankMSE" or (name == "ApproxNDCG" and bool(params.get("batch_coupled", True)))
     ranges = _launch_ranges(B, n, offsets, params.get("buckets"), coupled or not quadratic)
     if name == "ListMLE":
@@ -164,6 +171,11 @@ def _loss_call(name: str, scores: torch.Tensor, labels: torch.Tensor, params: di
         elif name == "SoftRank":
             top_k = params.get("top_k")
             rc = lib.ptrb200_softrank_fwd_bwd(sp, yp, opq, gp, lqq, Bq, nq, float(params.get("delta", 2.0)), int(top_k) if top_k else 0, st)
+        elif name == "WassRank":
+            # every launch divides by the query count of the whole batch, so buckets reproduce the single launch
+            rc = lib.ptrb200_wassrank_fwd_bwd(sp, yp, opq, gp, lqq, Bq, nq, B, _lib.WASS_COST_TYPES[cost], float(params.get("lam", 0.1)),
+                                              int(params.get("sh_itr", 20)), float(params.get("non_rele_gap", 100.0)),
+                                              float(params.get("var_penalty", math.e)), float(params.get("gain_base", 4.0)), st)
         else:
             raise NotImplementedError(name)
         _lib.check(rc, f"{name} loss kernel")

@@ -49,6 +49,9 @@ for name, params, shapes in [
     ("STListNet", dict(temperature=1.0), [(1024, 256), (4096, 32)]),
     ("RankCosine", {}, [(1024, 256)]),
     ("RankMSE", {}, [(1024, 256)]),
+    ("WassRank", dict(cost_type="eg"), [(1024, 256), (256, 1024)]),      # default settings: label-group schedule
+    ("WassRank", dict(cost_type="ddg"), [(1024, 256)]),                  # O(n^2) walks
+    ("WassRank", dict(cost_type="p1"), [(256, 1024)]),
 ]:
     for (B, n) in shapes:
         s = torch.sigmoid(torch.randn(B, n, device=dev))
@@ -60,7 +63,7 @@ for name, params, shapes in [
             kw.update(seed=1, offset=1)
         ms = timeit(lambda: ops.rank_loss_and_grad(name, s, y, **kw))
         algo = (16 if name == "ListMLE" else 12) * n * B
-        rows.append((f"{name} {params.get('loss_type', '')} {('k=%d' % params['k']) if 'k' in params else ''}".strip(), f"B={B} n={n}",
+        rows.append((f"{name} {params.get('loss_type', params.get('cost_type', ''))} {('k=%d' % params['k']) if 'k' in params else ''}".strip(), f"B={B} n={n}",
                      ms, B / ms * 1e3, algo / ms / 1e6, algo / ms / 1e6 / HBM))
 # ndcg / all metrics
 for (B, n) in [(1024, 256), (256, 1024)]:
@@ -103,6 +106,11 @@ for (B, n) in [(1024, 256), (256, 1024), (4096, 32)]:
     algo = n * B * (136 * 4 + 8)
     rows.append(("pointsf forward (5x100 GELU BN)", f"B={B} n={n}", ms_f, B / ms_f * 1e3, algo / ms_f / 1e6, algo / ms_f / 1e6 / HBM))
     rows.append(("LambdaRank train step (fwd+loss+bwd+Adam)", f"B={B} n={n}", ms_s, B / ms_s * 1e3, algo / ms_s / 1e6, algo / ms_s / 1e6 / HBM))
+    if (B, n) == (1024, 256):       # the same step with WassRank's default settings (eg cost, lam 0.1, 20 iterations)
+        rw = ptranking_b200.WassRank(sf_para_dict=sf, wass_para_dict=None, dict_cost_mats={}, dict_std_dists={}, gpu=True, device=dev)
+        rw.init(); rw.train_mode()
+        ms_w = timeit(lambda: rw.train_op(X, y, presort=True, label_type=LABEL_TYPE.MultiLabel, epoch_k=1))
+        rows.append(("WassRank train step (fwd+loss+bwd+Adam)", f"B={B} n={n}", ms_w, B / ms_w * 1e3, algo / ms_w / 1e6, algo / ms_w / 1e6 / HBM))
 # the same step on the ragged batch (batch-level BN: one long list to the scorer, per-query offsets to the loss)
 Xr = torch.randn(total, 136, device=dev)
 ms_s = timeit(lambda: r.train_op(Xr, y_r, presort=True, label_type=LABEL_TYPE.MultiLabel, epoch_k=1, offsets=off_d, max_len=int(lens.max()), buckets=buckets))
