@@ -239,12 +239,13 @@ def stlistnet(s, y, unif, temperature=1.0):
 
 def softrank(s, y, delta=2.0, top_k=None):
     """listwise/softrank.py:46-72 (nDCG, labels presorted)."""
-    from math import erfc, pi, sqrt
+    from math import pi, sqrt
+    from scipy.special import erfc
     s = s.astype(np.float64); y = y.astype(np.float64)
     B, n = s.shape
     den = sqrt(2.0 * 2.0 * delta * delta)
     x = (s[:, :, None] - s[:, None, :]) / den                       # [b,i,j]
-    phi = 0.5 * np.vectorize(erfc)(x)
+    phi = 0.5 * erfc(x)
     off = 1.0 - np.eye(n)[None]
     r = (phi * off).sum(2) + 1.0
     G = _gain(y)

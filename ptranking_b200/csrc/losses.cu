@@ -22,6 +22,11 @@ namespace ptrb200 {
 // Thread-per-row: the thread owning sorted position i visits every j != i and
 // evaluates the ordered pair (min(i,j), max(i,j)) exactly as the reference's
 // upper-triangular tensors do, so no scatter / atomics are needed.
+// LambdaRank skips equal-label pairs, as lambdarank_runs_kernel does: their
+// weight |G_i - G_j| |1/D_i - 1/D_j| is exactly 0 and they add exactly +-0,
+// except in a list without a relevant document (iDCG = 0), where every
+// normalised gain is 0/0.  Skipping them there too gives such a list loss 0
+// and gradient 0 whichever kernel its launch picks.
 // ---------------------------------------------------------------------------
 template <bool LAMBDA>
 __global__ void pairwise_bce_kernel(const float* __restrict__ scores, const float* __restrict__ labels,
@@ -68,7 +73,7 @@ __global__ void pairwise_bce_kernel(const float* __restrict__ scores, const floa
         const float gi = LAMBDA ? ng[i] : 0.0f, di = LAMBDA ? dinv[i] : 0.0f;
         float acc = 0.0f;
         for (int j = 0; j < n; ++j) {
-            if (j == i) continue;
+            if (j == i || (LAMBDA && yi == ys[j])) continue;
             const bool upper = j > i;
             float x = sigma * (si - ss[j]);
             float S = fminf(fmaxf(yi - ys[j], -1.0f), 1.0f);
