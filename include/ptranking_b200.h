@@ -51,7 +51,7 @@ int                ptrb200_version(void);
 const char*        ptrb200_last_error(void);
 /* number of kernels this library has launched in this process (bench.py's gpu_launches) */
 unsigned long long ptrb200_launch_count(void);
-/* 1 if the current device is compute capability 10.x (the only target built) */
+/* 1 if the current device is compute capability 9.0 (sm_90a, the only target built) */
 int                ptrb200_device_ok(void);
 /* Per-launch CUDA-event timing on the launching stream (bench.py's roofline pass; off by default).
  * ptrb200_timing_report synchronises the recorded events and writes one line per kernel,
@@ -178,6 +178,10 @@ int ptrb200_adhoc_metrics_at_ks(const float* scores, const float* labels, const 
  * :484-485).  In-place (out == X) is allowed. */
 int ptrb200_standard_scale(const float* X, const int32_t* offsets, float* out, int B, int n, int F,
                            int clip, float clip_max, ptrb200_stream_t stream);
+/* The same with bf16 output (raw bf16 bit patterns): the result is computed exactly as above in fp32 and rounded to nearest
+ * even at the store -- scaling first, because raw LETOR features lose precision in bf16.  out must not alias X. */
+int ptrb200_standard_scale_bf16(const float* X, const int32_t* offsets, uint16_t* out, int B, int n, int F,
+                                int clip, float clip_max, ptrb200_stream_t stream);
 
 /* ---- stacked feed-forward scorer (pointwise MLP; also the head/tail nets of listsf) ---- */
 /* get_stacked_FFNet, ptranking/base/utils.py:288-356; PointNeuralRanker.forward,
@@ -202,8 +206,15 @@ int ptrb200_standard_scale(const float* X, const int32_t* offsets, float* out, i
 #define PTRB200_MATH_TF32   2   /* wgmma tf32, single pass (10-bit mantissa operands)               */
 #define PTRB200_MATH_BF16   3   /* every GEMM operand (features, activations, weights, gradients) rounded to bf16
                                    (round-to-nearest-even), products exact, fp32 accumulation: the numerics of a bf16
-                                   tensor-core GEMM, issued as one tf32 wgmma pass (bf16 values are tf32 values);
-                                   tensors stay fp32 in memory.  Needs tensor-core-eligible widths (no SIMT fallback) */
+                                   tensor-core GEMM, issued as one tf32 wgmma pass (bf16 values are tf32 values).
+                                   Activations, weights and the workspace stay fp32 in memory; the features may be
+                                   bf16 in memory (the _x entries below, PTRB200_DTYPE_BF16), which halves their
+                                   reads.  Needs tensor-core-eligible widths (no SIMT fallback) */
+
+/* Element type of the feature matrix X in the ptrb200_ffnet_*_x entries.  A bf16 X gives bit for bit the results of the
+ * same values passed as fp32 (bf16 values are exact in fp32 and tf32), in every math mode. */
+#define PTRB200_DTYPE_F32  0
+#define PTRB200_DTYPE_BF16 1   /* raw bf16 bit patterns, 8-byte aligned, row pitch dims[0] elements */
 
 typedef struct ptrb200_ffnet {
     int num_linear;                        /* linear layers, output layer included            */
@@ -273,6 +284,20 @@ int ptrb200_ffnet_backward(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* 
                            const float* dOut, float* dX, void* workspace, int64_t workspace_bytes,
                            int B, int n, const int32_t* offsets, int total_rows, int training, uint64_t seed, uint64_t offset,
                            ptrb200_stream_t stream);
+
+/* The three calls above with the feature element type as an argument (x_dtype = PTRB200_DTYPE_*; the calls above are
+ * these with PTRB200_DTYPE_F32).  A bf16 X is read natively by layer 0's tensor-core kernels (forward and weight
+ * gradient, half the feature bytes, no fp32 copy); a feature width that is not a multiple of 4 and math_mode SIMT widen
+ * it once into the workspace instead.  dX stays fp32.  An unknown x_dtype or a bf16 X that is not 8-byte aligned returns
+ * PTRB200_ERR_INVALID.  The workspace size depends on x_dtype: size it with the _x call. */
+int64_t ptrb200_ffnet_workspace_bytes_x(const ptrb200_ffnet* net, int x_dtype, int B, int n, int total_rows);
+int ptrb200_ffnet_forward_x(const ptrb200_ffnet* net, const void* X, int x_dtype, float* out, void* workspace,
+                            int64_t workspace_bytes, int B, int n, const int32_t* offsets, int total_rows, int training,
+                            uint64_t seed, uint64_t offset, ptrb200_stream_t stream);
+int ptrb200_ffnet_backward_x(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, const void* X, int x_dtype,
+                             const float* dOut, float* dX, void* workspace, int64_t workspace_bytes,
+                             int B, int n, const int32_t* offsets, int total_rows, int training, uint64_t seed, uint64_t offset,
+                             ptrb200_stream_t stream);
 
 /* ---- optimizer step ---------------------------------------------------------------------- */
 /* torch.optim.Adam.step() (ranker.py:512-525 -> config_optimizer; defaults betas=(0.9,0.999), eps=1e-8) over flat fp32

@@ -20,6 +20,7 @@ NORM_CODES = {None: 0, "BN": 1, "BN2": 2}
 MATH_MODES = {"simt": 0, "3xtf32": 1, "tf32": 2, "bf16": 3}
 LAMBDALOSS_TYPES = {"NDCG_Loss1": 0, "NDCG_Loss2": 1, "NDCG_Loss2++": 2}
 WASS_COST_TYPES = {"p1": 0, "p2": 1, "eg": 2, "dg": 3, "ddg": 4}   # PTRB200_WASS_COST_*
+DTYPE_F32, DTYPE_BF16 = 0, 1                                       # PTRB200_DTYPE_*: feature element type of the _x entries
 
 _fp = C.c_void_p   # device pointers travel as integers
 
@@ -97,6 +98,11 @@ SIGNATURES = {
     "ptrb200_ffnet_forward": (_I, [C.POINTER(FFNetDesc), _fp, _fp, _fp, _I64, _I, _I, _fp, _I, _I, _U64, _U64, _fp]),
     "ptrb200_ffnet_backward": (_I, [C.POINTER(FFNetDesc), C.POINTER(FFNetGrads), _fp, _fp, _fp, _fp, _I64,
                                     _I, _I, _fp, _I, _I, _U64, _U64, _fp]),
+    "ptrb200_standard_scale_bf16": (_I, [_fp, _fp, _fp, _I, _I, _I, _I, _F, _fp]),
+    "ptrb200_ffnet_workspace_bytes_x": (_I64, [C.POINTER(FFNetDesc), _I, _I, _I, _I]),
+    "ptrb200_ffnet_forward_x": (_I, [C.POINTER(FFNetDesc), _fp, _I, _fp, _fp, _I64, _I, _I, _fp, _I, _I, _U64, _U64, _fp]),
+    "ptrb200_ffnet_backward_x": (_I, [C.POINTER(FFNetDesc), C.POINTER(FFNetGrads), _fp, _I, _fp, _fp, _fp, _I64,
+                                      _I, _I, _fp, _I, _I, _U64, _U64, _fp]),
 }
 
 MAX_PEERS = 16

@@ -182,8 +182,11 @@ class ListNeuralRanker(NeuralRanker):
                 'tail_ffnns': tail_ffnns.to(self.device)}
 
     def forward(self, batch_q_doc_vectors):
-        """[B,n,F] -> [B,n] (list_ranker.py:351-378)."""
+        """[B,n,F] -> [B,n] (list_ranker.py:351-378).  bf16 features are upcast to fp32 here: the encoder and the
+        DASALC / AttnDIN glue consume X in fp32 (only the pointwise scorer reads bf16 features natively)."""
         X = batch_q_doc_vectors
+        if X.dtype != torch.float32:
+            X = X.float()
         head, enc, tail = self.list_sf['head_ffnns'], self.list_sf['encoder'], self.list_sf['tail_ffnns']
         if 'AllRank' == self.encoder_type:
             z = enc(head(X))

@@ -3,6 +3,8 @@
 // Reference functions replaced (wildltr/ptranking @ f1d366c):
 //   per-query feature scaling  ptranking/data/data_utils.py:482-487 (sklearn StandardScaler().fit_transform per query,
 //                              ISTELLA clip at :484-485; which datasets are scaled: :205-218)
+#include <cuda_bf16.h>
+
 #include "losses_common.cuh"
 
 namespace ptrb200 {
@@ -11,14 +13,19 @@ namespace ptrb200 {
 // sklearn semantics: mean over the query's documents, POPULATION variance (ddof = 0), both accumulated in float64
 // (two passes: the variance is the mean squared deviation from the computed mean); a constant column -- variance not
 // above sklearn's _is_constant_feature bound n*eps*var + (n*mean*eps)^2 -- is divided by 1 instead of 0.
-__global__ void standard_scale_kernel(const float* __restrict__ X, const int32_t* __restrict__ offsets, float* __restrict__ out,
-                                      int n_uniform, int F, float clip_max, int clip) {
+// OutT = uint16_t: bf16 output, the fp32 result rounded to nearest even at the store.
+static __device__ __forceinline__ float to_out(float v, float*) { return v; }
+static __device__ __forceinline__ uint16_t to_out(float v, uint16_t*) { return __bfloat16_as_ushort(__float2bfloat16_rn(v)); }
+
+template <typename OutT>
+static __device__ __forceinline__ void standard_scale_query(const float* __restrict__ X, const int32_t* __restrict__ offsets,
+                                                            OutT* __restrict__ out, int n_uniform, int F, float clip_max, int clip) {
     const int b = blockIdx.x;
     const ListSpan sp = list_span(offsets, b, n_uniform);
     const int n = sp.n;
     if (n == 0) return;
     const float* x = X + sp.base * (size_t)F;
-    float* o = out + sp.base * (size_t)F;
+    OutT* o = out + sp.base * (size_t)F;
     for (int f = threadIdx.x; f < F; f += blockDim.x) {
         double s = 0.0;
         for (int r = 0; r < n; ++r) { float v = x[(size_t)r * F + f]; if (clip) v = fminf(v, clip_max); s += (double)v; }
@@ -32,9 +39,17 @@ __global__ void standard_scale_kernel(const float* __restrict__ X, const int32_t
         for (int r = 0; r < n; ++r) {
             float v = x[(size_t)r * F + f];
             if (clip) v = fminf(v, clip_max);
-            o[(size_t)r * F + f] = (float)(((double)v - mean) / scale);
+            o[(size_t)r * F + f] = to_out((float)(((double)v - mean) / scale), o);
         }
     }
+}
+__global__ void standard_scale_kernel(const float* __restrict__ X, const int32_t* __restrict__ offsets, float* __restrict__ out,
+                                      int n_uniform, int F, float clip_max, int clip) {
+    standard_scale_query(X, offsets, out, n_uniform, F, clip_max, clip);
+}
+__global__ void standard_scale_bf16_kernel(const float* __restrict__ X, const int32_t* __restrict__ offsets, uint16_t* __restrict__ out,
+                                           int n_uniform, int F, float clip_max, int clip) {
+    standard_scale_query(X, offsets, out, n_uniform, F, clip_max, clip);
 }
 
 // Ragged <-> padded: the list scorer's attention works on dense [B, n_max, .] tensors; a ragged batch (flat rows + prefix
@@ -80,4 +95,13 @@ extern "C" int ptrb200_standard_scale(const float* X, const int32_t* offsets, fl
     int threads = ((F + 31) / 32) * 32; if (threads > 256) threads = 256;
     PTRB200_LAUNCH(standard_scale_kernel, B, threads, 0, stream, X, offsets, out, n, F, clip_max, clip);
     return check_launch("standard_scale");
+}
+
+extern "C" int ptrb200_standard_scale_bf16(const float* X, const int32_t* offsets, uint16_t* out, int B, int n, int F,
+                                           int clip, float clip_max, ptrb200_stream_t stream) {
+    if (!X || !out || B <= 0 || n <= 0 || F <= 0) { set_error("standard_scale_bf16: bad arguments (B=%d n=%d F=%d)", B, n, F); return PTRB200_ERR_INVALID; }
+    if ((const void*)X == (const void*)out) { set_error("standard_scale_bf16: out must not alias X"); return PTRB200_ERR_INVALID; }
+    int threads = ((F + 31) / 32) * 32; if (threads > 256) threads = 256;
+    PTRB200_LAUNCH(standard_scale_bf16_kernel, B, threads, 0, stream, X, offsets, out, n, F, clip_max, clip);
+    return check_launch("standard_scale_bf16");
 }

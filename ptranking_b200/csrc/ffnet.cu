@@ -623,6 +623,10 @@ struct Plan {
     bool ragged;                                 // per-query BN2 over a ragged batch (query boundaries from prefix offsets)
     int pad_k;                                   // > 0: input width zero-padded to this multiple of 4 for the tensor-core path
     size_t xpad_off, w0pad_off, dw0pad_off, dxpad_off;
+    // bf16 features (PTRB200_DTYPE_BF16): read natively by the layer-0 tensor-core kernels; the padded and SIMT paths
+    // widen them once into an fp32 workspace copy (xpad_off resp. xwide_off) and run unchanged
+    bool x_bf16;
+    size_t xwide_off;
 };
 
 // column blocking of the weight gradient: dZ columns in blocks of 128 (two m64 MMA tiles), input columns in blocks of <= 256
@@ -637,8 +641,10 @@ static WgBlocks wgrad_blocks(int N, int K) {
     return b;
 }
 
-static int make_plan(const ptrb200_ffnet* net, int B, int n, Plan& p, int total_rows = 0) {
+static int make_plan(const ptrb200_ffnet* net, int B, int n, Plan& p, int total_rows = 0, int x_dtype = PTRB200_DTYPE_F32) {
     if (!net || B <= 0 || n <= 0 || total_rows < 0) { set_error("ffnet: null net or non-positive B/n"); return PTRB200_ERR_INVALID; }
+    if (x_dtype != PTRB200_DTYPE_F32 && x_dtype != PTRB200_DTYPE_BF16) { set_error("ffnet: unknown feature dtype code %d", x_dtype); return PTRB200_ERR_INVALID; }
+    p.x_bf16 = x_dtype == PTRB200_DTYPE_BF16;
     if (net->num_linear < 1 || net->num_linear > PTRB200_MAX_FF_LAYERS) { set_error("ffnet: num_linear=%d outside 1..%d", net->num_linear, PTRB200_MAX_FF_LAYERS); return PTRB200_ERR_INVALID; }
     if (net->norm < PTRB200_NORM_NONE || net->norm > PTRB200_NORM_BN2) { set_error("ffnet: bad norm %d", net->norm); return PTRB200_ERR_INVALID; }
     if (!(net->dropout_p >= 0.0f && net->dropout_p < 1.0f)) { set_error("ffnet: dropout_p must be in [0,1)"); return PTRB200_ERR_INVALID; }
@@ -740,6 +746,8 @@ static int make_plan(const ptrb200_ffnet* net, int B, int n, Plan& p, int total_
         p.dw0pad_off = off; off = align_up(off + (size_t)net->dims[1] * p.pad_k * 4, 256);
         p.dxpad_off = off; off = align_up(off + p.rows * p.pad_k * 4, 256);
     }
+    p.xwide_off = off;
+    if (p.x_bf16 && !p.use_tc) { p.xwide_off = off; off = align_up(off + p.rows * (size_t)net->dims[0] * 4, 256); }
     p.total = off;
     return PTRB200_OK;
 }
@@ -813,6 +821,16 @@ __global__ void copy_cols_kernel(const float* __restrict__ src, float* __restric
         dst[i] = k < ks ? src[r * ks + k] : 0.0f;
     }
 }
+// the same from bf16 features (exact widening): the padded fp32 copy of a bf16 feature matrix (ks % 4 != 0), and with
+// kd == ks the fp32 copy the SIMT kernels read
+__global__ void copy_cols_bf16_kernel(const uint16_t* __restrict__ src, float* __restrict__ dst, size_t rows, int ks, int kd) {
+    const size_t total = rows * (size_t)kd;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t r = i / kd;
+        const int k = (int)(i - r * kd);
+        dst[i] = k < ks ? __uint_as_float((uint32_t)src[r * ks + k] << 16) : 0.0f;
+    }
+}
 
 // ------------------------------------------------------------------ tensor-core host paths
 
@@ -856,10 +874,12 @@ static bool rows_ws_fits(int K, int N, int passes) {
 
 // stats_kind: 0 none, 1 one statistics group over the whole batch (BN), 2 per-query groups (BN2).
 // *S_out receives the number of partial slots per group the kernel wrote.
+// xb: g.P holds bf16 features -- layer 0's forward (no scale/shift, no activation), the kernels' XB variants.
 static int launch_rows_gemm(int mode, int passes, RowsGemmArgs& g, int ntiles, cudaStream_t st,
-                            int stats_kind = 0, int* S_out = nullptr, int S_default = 1) {
+                            int stats_kind = 0, int* S_out = nullptr, int S_default = 1, bool xb = false) {
     g.NP = ((g.N + 15) / 16) * 16;
     int rc;
+    if (xb && (mode != RG_FWD || g.scale || g.act != PTRB200_AF_NONE)) { set_error("rows_gemm: bf16 input only feeds layer 0's forward"); return PTRB200_ERR_INVALID; }
     const int nchunks = (g.K + 31) / 32;
     // ---- persistent warp-specialised kernel when the whole weight image fits beside the A ring ----
     const size_t ws_smem = 1024 + (size_t)nchunks * g.NP * 128 * (passes == 3 ? 2 : 1) + 65536 + (size_t)RW_EPI_WARPS * g.NP * 8 + 128;
@@ -884,6 +904,18 @@ static int launch_rows_gemm(int mode, int passes, RowsGemmArgs& g, int ntiles, c
         }
         // the prologue activation is a template parameter for the common codes, -1 = generic run-time switch
         const int act_t = (g.act == PTRB200_AF_NONE || g.act == PTRB200_AF_RELU || g.act == PTRB200_AF_GELU || g.act == PTRB200_AF_SIGM) ? g.act : -1;
+        if (xb) {
+#define RWX_CASE(P, KT)                                                                                           \
+            if (passes == P && (KT == 0 || g.K == KT)) {                                                          \
+                if ((rc = opt_in_smem(rows_gemm_ws_kernel<RG_FWD, P, PTRB200_AF_NONE, KT, true>, ws_smem))) return rc; \
+                PTRB200_LAUNCH_TAG("rows_gemm_ws_fwd_xbf16", (rows_gemm_ws_kernel<RG_FWD, P, PTRB200_AF_NONE, KT, true>), grid, RW_THREADS, ws_smem, st, g, x); \
+                return PTRB200_OK;                                                                                \
+            }
+            RWX_CASE(3, 136) RWX_CASE(1, 136) RWX_CASE(3, 0) RWX_CASE(1, 0)
+#undef RWX_CASE
+            set_error("rows_gemm: no bf16-input variant for %d passes", passes);
+            return PTRB200_ERR_INVALID;
+        }
         // width-specialised instantiations for the default scorer (136 features, 100-wide hidden layers)
         RW_CASE_K(RG_FWD, 3, PTRB200_AF_NONE, 136, "rows_gemm_ws_fwd") RW_CASE_K(RG_FWD, 3, PTRB200_AF_GELU, 100, "rows_gemm_ws_fwd")
         RW_CASE_K(RG_DGRAD, 3, PTRB200_AF_NONE, 100, "rows_gemm_ws_dgrad")
@@ -911,6 +943,16 @@ static int launch_rows_gemm(int mode, int passes, RowsGemmArgs& g, int ntiles, c
     g.tail_off = (int)(((operands > otile ? operands : otile) + 15) / 16 * 16);
     const size_t smem = 1024 + (size_t)g.tail_off + 64;
     const dim3 rg_grid(ntiles, n_tiles);
+    if (xb) {
+        if (passes == 3) {
+            if ((rc = opt_in_smem(rows_gemm_tc_kernel<RG_FWD, 3, PTRB200_AF_NONE, true>, smem))) return rc;
+            PTRB200_LAUNCH_TAG("rows_gemm_tc_fwd_xbf16", (rows_gemm_tc_kernel<RG_FWD, 3, PTRB200_AF_NONE, true>), rg_grid, RG_THREADS, smem, st, g);
+        } else {
+            if ((rc = opt_in_smem(rows_gemm_tc_kernel<RG_FWD, 1, -1, true>, smem))) return rc;
+            PTRB200_LAUNCH_TAG("rows_gemm_tc_fwd_xbf16", (rows_gemm_tc_kernel<RG_FWD, 1, -1, true>), rg_grid, RG_THREADS, smem, st, g);
+        }
+        return PTRB200_OK;
+    }
     // the prologue's activation as a compile-time constant for the common cases (a runtime switch per element is what the
     // ncu capture of the 256 -> 512 head layer showed: 65 thread instructions per staged element)
 #define RG_CASE(M, P, A, TAG)                                                                      \
@@ -1064,14 +1106,25 @@ static void pack_weight_images(const ptrb200_ffnet* net, const Plan& p, char* ws
 // dW[N,K] = sum_rows dZ^T (x) P on tensor cores.  The caller fills the operands of w (dZ, P, dropout, partials, rows and,
 // for the folded normalisation backward, Z2 and the coefficients); grid.x persistent CTAs per (dZ block, input block)
 // each write one partial, which reduce_splits_kernel sums in a fixed order.
-static int launch_wgrad(WgradArgs& w, int N, int K, int kb, dim3 grid, int passes, float* dW, cudaStream_t st) {
+// xb: w.P holds bf16 features (layer 0).  The tile height -- and with it the rows every CTA sums and the order of the
+// partials -- is the one the fp32 layer input gets, so both give the same dW bit for bit; only the raw ring shrinks.
+static int launch_wgrad(WgradArgs& w, int N, int K, int kb, dim3 grid, int passes, float* dW, cudaStream_t st, bool xb = false) {
     int rc;
     const bool fused_dz = w.Z2 != nullptr;
     w.N_full = N; w.K_full = K; w.kb = kb;
     w.N = N < 128 ? N : 128; w.K = kb;       // block maxima (buffer geometry)
     w.KP = ((w.K + 15) / 16) * 16;
-    const size_t smem = wgrad_smem(w.N, w.K, w.KP, w.tile_rows, passes, w.stages, fused_dz, fused_dz ? 24 : 8);
-    if (passes == 3) { if ((rc = opt_in_smem(wgrad_tc_kernel<3>, smem))) return rc; PTRB200_LAUNCH_TAG("wgrad_tc", wgrad_tc_kernel<3>, grid, WG_THREADS, smem, st, w); }
+    size_t smem = wgrad_smem(w.N, w.K, w.KP, w.tile_rows, passes, w.stages, fused_dz, fused_dz ? 24 : 8);
+    if (xb) {
+        // the kernel's layout at the same tile height and ring depth, with the layer-input slots at 2 bytes per element
+        const size_t op = (size_t)(128 + w.KP) * 128 * (passes == 3 ? 2 : 1);
+        const size_t rawz = (((size_t)w.tile_rows * w.N * 4 + 127) / 128 * 128) * (fused_dz ? 2 : 1);
+        const size_t rawp = ((size_t)w.tile_rows * w.K * 2 + 127) / 128 * 128;
+        smem = 1024 + 2 * op + 128 + 3 * 128 * 4 + (size_t)w.stages * (rawz + rawp);
+        if (passes == 3) { if ((rc = opt_in_smem(wgrad_tc_kernel<3, true>, smem))) return rc; PTRB200_LAUNCH_TAG("wgrad_tc_xbf16", (wgrad_tc_kernel<3, true>), grid, WG_THREADS, smem, st, w); }
+        else { if ((rc = opt_in_smem(wgrad_tc_kernel<1, true>, smem))) return rc; PTRB200_LAUNCH_TAG("wgrad_tc_xbf16", (wgrad_tc_kernel<1, true>), grid, WG_THREADS, smem, st, w); }
+    }
+    else if (passes == 3) { if ((rc = opt_in_smem(wgrad_tc_kernel<3>, smem))) return rc; PTRB200_LAUNCH_TAG("wgrad_tc", wgrad_tc_kernel<3>, grid, WG_THREADS, smem, st, w); }
     else { if ((rc = opt_in_smem(wgrad_tc_kernel<1>, smem))) return rc; PTRB200_LAUNCH_TAG("wgrad_tc", wgrad_tc_kernel<1>, grid, WG_THREADS, smem, st, w); }
     PTRB200_LAUNCH(reduce_splits_kernel, (N * K + 63) / 64, 256, 0, st, (const float*)w.partials, dW, (int)grid.x, N * K);
     return PTRB200_OK;
@@ -1125,7 +1178,8 @@ static void set_norm_grads(DyTail& t, const ptrb200_ffnet* net, const ptrb200_ff
 // Dense and ragged plans share the contractions; p.ragged (per-query BN2 over a ragged batch) only changes the
 // normalisation step: per-query bn2_ragged_* kernels on a materialised layer input instead of the epilogue statistics
 // partials and the normalisation folded into the next layer's prologue.
-static int forward_tc(const ptrb200_ffnet* net, const Plan& p, const float* X, const int32_t* offsets, float* out, char* ws,
+// xb: X holds bf16 features, read natively by layer 0's forward and weight-gradient kernels.
+static int forward_tc(const ptrb200_ffnet* net, const Plan& p, const float* X, bool xb, const int32_t* offsets, float* out, char* ws,
                       float drop, uint64_t seed, uint64_t offset, cudaStream_t st, bool fwd_only) {
     int rc;
     pack_weight_images(net, p, ws, fwd_only, st);
@@ -1147,7 +1201,7 @@ static int forward_tc(const ptrb200_ffnet* net, const Plan& p, const float* X, c
         set_tiling(g, p);
         int S_fwd = p.S_stat;
         const int stats_kind = !g.partials ? 0 : (net->norm == PTRB200_NORM_BN ? 1 : 2);
-        if ((rc = launch_rows_gemm(RG_FWD, p.passes, g, p.ntiles, st, stats_kind, &S_fwd, p.S_stat))) return rc;
+        if ((rc = launch_rows_gemm(RG_FWD, p.passes, g, p.ntiles, st, stats_kind, &S_fwd, p.S_stat, xb && l == 0))) return rc;
         NormRef nr = norm_ref(net, p, l, ws);
         if (p.ragged) {
             if (lp.has_norm) {      // (under BN2 every layer with an activation has a norm)
@@ -1181,7 +1235,7 @@ static int forward_tc(const ptrb200_ffnet* net, const Plan& p, const float* X, c
     return check_launch("ffnet_forward(tc)");
 }
 
-static int backward_tc(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, const Plan& p, const float* X, const int32_t* offsets,
+static int backward_tc(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, const Plan& p, const float* X, bool xb, const int32_t* offsets,
                        const float* dOut, float* dX, char* ws, float drop, uint64_t seed, uint64_t offset, cudaStream_t st) {
     int rc;
     double* part = reinterpret_cast<double*>(ws + p.partials_off);
@@ -1261,7 +1315,7 @@ static int backward_tc(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grad
                 w.kc1 = reinterpret_cast<const float*>(ws + p.k1_off); w.kc3 = reinterpret_cast<const float*>(ws + p.k3_off); w.kc0 = reinterpret_cast<const float*>(ws + p.k0_off);
             }
             const WgBlocks wb = wgrad_blocks(lp.d_out, lp.d_in);
-            if ((rc = launch_wgrad(w, lp.d_out, lp.d_in, wb.kb, dim3(wb.gx, wb.mblocks, wb.kblocks), p.passes, grads->weight[l], st))) return rc;
+            if ((rc = launch_wgrad(w, lp.d_out, lp.d_in, wb.kb, dim3(wb.gx, wb.mblocks, wb.kblocks), p.passes, grads->weight[l], st, xb && l == 0))) return rc;
             // every parameter gradient of layer l is now enqueued: a data-parallel caller can start reducing it while the
             // layers below are still running (dist.GradBucket's overlapped all-reduce)
             if ((rc = call_hook(PTRB200_HOOK_LAYER_GRADS_READY, l, nullptr, 0, st))) return rc;
@@ -1310,34 +1364,55 @@ int ptrb200_tc_wgrad(const float* dZ, const float* P, float* dW, float* partials
     return rc ? rc : check_launch("tc_wgrad");
 }
 
-int64_t ptrb200_ffnet_workspace_bytes(const ptrb200_ffnet* net, int B, int n, int total_rows) {
+int64_t ptrb200_ffnet_workspace_bytes_x(const ptrb200_ffnet* net, int x_dtype, int B, int n, int total_rows) {
     Plan p;
-    const int rc = make_plan(net, B, n, p, total_rows);
+    const int rc = make_plan(net, B, n, p, total_rows, x_dtype);
     return rc ? (int64_t)rc : (int64_t)p.total;
 }
 
-int ptrb200_ffnet_forward(const ptrb200_ffnet* net, const float* X, float* out, void* workspace,
-                          int64_t workspace_bytes, int B, int n, const int32_t* offsets, int total_rows, int training,
-                          uint64_t seed, uint64_t offset, ptrb200_stream_t stream) {
+int64_t ptrb200_ffnet_workspace_bytes(const ptrb200_ffnet* net, int B, int n, int total_rows) {
+    return ptrb200_ffnet_workspace_bytes_x(net, PTRB200_DTYPE_F32, B, n, total_rows);
+}
+
+// a bf16 feature matrix is read 4 elements (8 bytes) at a time
+static int check_x(const void* X, int x_dtype, const char* who) {
+    if (x_dtype == PTRB200_DTYPE_BF16 && (reinterpret_cast<uintptr_t>(X) & 7) != 0) {
+        set_error("%s: bf16 features must be 8-byte aligned (X = %p)", who, X);
+        return PTRB200_ERR_INVALID;
+    }
+    return PTRB200_OK;
+}
+
+int ptrb200_ffnet_forward_x(const ptrb200_ffnet* net, const void* Xv, int x_dtype, float* out, void* workspace,
+                            int64_t workspace_bytes, int B, int n, const int32_t* offsets, int total_rows, int training,
+                            uint64_t seed, uint64_t offset, ptrb200_stream_t stream) {
     Plan p;
     if ((offsets != nullptr) != (total_rows > 0)) { set_error("ffnet_forward: offsets and total_rows go together (ragged batch) or are both absent"); return PTRB200_ERR_INVALID; }
-    int rc = make_plan(net, B, n, p, total_rows);
+    int rc = make_plan(net, B, n, p, total_rows, x_dtype);
     if (rc) return rc;
-    if (!X || !out || !workspace) { set_error("ffnet_forward: null buffer"); return PTRB200_ERR_INVALID; }
+    if (!Xv || !out || !workspace) { set_error("ffnet_forward: null buffer"); return PTRB200_ERR_INVALID; }
+    if ((rc = check_x(Xv, x_dtype, "ffnet_forward"))) return rc;
     if ((size_t)workspace_bytes < p.total) { set_error("ffnet_forward: workspace %lld < %zu bytes", (long long)workspace_bytes, p.total); return PTRB200_ERR_WORKSPACE; }
     char* ws = static_cast<char*>(workspace);
     cudaStream_t st = (cudaStream_t)stream;
     const float drop = (training & 1) ? net->dropout_p : 0.0f;
+    const float* X = static_cast<const float*>(Xv);       // bf16: reinterpreted by the kernels that read it (xb)
+    bool xb = p.x_bf16;
     ptrb200_ffnet padded;
     if (p.pad_k) {          // zero-pad the features and the first weight matrix to a multiple of 4 columns (make_plan)
         float* Xp = reinterpret_cast<float*>(ws + p.xpad_off);
         float* Wp = reinterpret_cast<float*>(ws + p.w0pad_off);
-        PTRB200_LAUNCH(copy_cols_kernel, elementwise_blocks(p.rows * p.pad_k), 256, 0, st, X, Xp, p.rows, net->dims[0], p.pad_k);
+        if (xb) PTRB200_LAUNCH(copy_cols_bf16_kernel, elementwise_blocks(p.rows * p.pad_k), 256, 0, st, static_cast<const uint16_t*>(Xv), Xp, p.rows, net->dims[0], p.pad_k);
+        else PTRB200_LAUNCH(copy_cols_kernel, elementwise_blocks(p.rows * p.pad_k), 256, 0, st, X, Xp, p.rows, net->dims[0], p.pad_k);
         PTRB200_LAUNCH(copy_cols_kernel, elementwise_blocks((size_t)net->dims[1] * p.pad_k), 256, 0, st, net->weight[0], Wp, (size_t)net->dims[1], net->dims[0], p.pad_k);
         padded = *net; padded.dims[0] = p.pad_k; padded.weight[0] = Wp;
-        net = &padded; X = Xp;
+        net = &padded; X = Xp; xb = false;
+    } else if (xb && !p.use_tc) {       // the SIMT kernels read fp32: widen once into the workspace (backward reads it too)
+        float* Xw = reinterpret_cast<float*>(ws + p.xwide_off);
+        PTRB200_LAUNCH(copy_cols_bf16_kernel, elementwise_blocks(p.rows * net->dims[0]), 256, 0, st, static_cast<const uint16_t*>(Xv), Xw, p.rows, net->dims[0], net->dims[0]);
+        X = Xw; xb = false;
     }
-    if (p.use_tc) return forward_tc(net, p, X, offsets, out, ws, drop, seed, offset, st, (training & PTRB200_FFNET_FORWARD_ONLY) != 0);
+    if (p.use_tc) return forward_tc(net, p, X, xb, offsets, out, ws, drop, seed, offset, st, (training & PTRB200_FFNET_FORWARD_ONLY) != 0);
     const float* in = X;
     for (int l = 0; l < p.L; ++l) {
         const LayerPlan& lp = p.layer[l];
@@ -1371,16 +1446,29 @@ int ptrb200_ffnet_forward(const ptrb200_ffnet* net, const float* X, float* out, 
     return check_launch("ffnet_forward");
 }
 
-int ptrb200_ffnet_backward(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, const float* X,
-                           const float* dOut, float* dX, void* workspace, int64_t workspace_bytes,
-                           int B, int n, const int32_t* offsets, int total_rows, int training, uint64_t seed, uint64_t offset,
-                           ptrb200_stream_t stream) {
+int ptrb200_ffnet_forward(const ptrb200_ffnet* net, const float* X, float* out, void* workspace,
+                          int64_t workspace_bytes, int B, int n, const int32_t* offsets, int total_rows, int training,
+                          uint64_t seed, uint64_t offset, ptrb200_stream_t stream) {
+    return ptrb200_ffnet_forward_x(net, X, PTRB200_DTYPE_F32, out, workspace, workspace_bytes, B, n, offsets, total_rows, training,
+                                   seed, offset, stream);
+}
+
+int ptrb200_ffnet_backward_x(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, const void* Xv, int x_dtype,
+                             const float* dOut, float* dX, void* workspace, int64_t workspace_bytes,
+                             int B, int n, const int32_t* offsets, int total_rows, int training, uint64_t seed, uint64_t offset,
+                             ptrb200_stream_t stream) {
     Plan p;
     if ((offsets != nullptr) != (total_rows > 0)) { set_error("ffnet_backward: offsets and total_rows go together (ragged batch) or are both absent"); return PTRB200_ERR_INVALID; }
-    int rc = make_plan(net, B, n, p, total_rows);
+    int rc = make_plan(net, B, n, p, total_rows, x_dtype);
     if (rc) return rc;
-    if (!grads || !X || !dOut || !workspace) { set_error("ffnet_backward: null buffer"); return PTRB200_ERR_INVALID; }
+    if (!grads || !Xv || !dOut || !workspace) { set_error("ffnet_backward: null buffer"); return PTRB200_ERR_INVALID; }
+    if ((rc = check_x(Xv, x_dtype, "ffnet_backward"))) return rc;
     if ((size_t)workspace_bytes < p.total) { set_error("ffnet_backward: workspace %lld < %zu bytes", (long long)workspace_bytes, p.total); return PTRB200_ERR_WORKSPACE; }
+    // bf16 features: layer 0's weight-gradient kernel reads them natively on the tensor-core path; the padded and the
+    // SIMT path read the fp32 copy the forward call left in the workspace
+    const float* X = p.x_bf16 && !p.use_tc ? reinterpret_cast<const float*>(static_cast<char*>(workspace) + p.xwide_off)
+                                           : static_cast<const float*>(Xv);
+    const bool xb = p.x_bf16 && p.use_tc && !p.pad_k;
     char* ws = static_cast<char*>(workspace);
     cudaStream_t st = (cudaStream_t)stream;
     const float drop = (training & 1) ? net->dropout_p : 0.0f;
@@ -1391,14 +1479,14 @@ int ptrb200_ffnet_backward(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* 
         pg.weight[0] = reinterpret_cast<float*>(ws + p.dw0pad_off);
         float* dXp = dX ? reinterpret_cast<float*>(ws + p.dxpad_off) : nullptr;
         const float* Xp = reinterpret_cast<const float*>(ws + p.xpad_off);
-        if ((rc = backward_tc(&padded, &pg, p, Xp, offsets, dOut, dXp, ws, drop, seed, offset, st))) return rc;
+        if ((rc = backward_tc(&padded, &pg, p, Xp, false, offsets, dOut, dXp, ws, drop, seed, offset, st))) return rc;
         if (!grads->weight[0]) { set_error("ffnet_backward: layer 0 grad buffer NULL"); return PTRB200_ERR_INVALID; }
         PTRB200_LAUNCH(copy_cols_kernel, elementwise_blocks((size_t)net->dims[1] * net->dims[0]), 256, 0, st, (const float*)pg.weight[0], grads->weight[0],
                        (size_t)net->dims[1], p.pad_k, net->dims[0]);
         if (dX) PTRB200_LAUNCH(copy_cols_kernel, elementwise_blocks(p.rows * net->dims[0]), 256, 0, st, (const float*)dXp, dX, p.rows, p.pad_k, net->dims[0]);
         return check_launch("ffnet_backward(padded)");
     }
-    if (p.use_tc) return backward_tc(net, grads, p, X, offsets, dOut, dX, ws, drop, seed, offset, st);
+    if (p.use_tc) return backward_tc(net, grads, p, X, xb, offsets, dOut, dX, ws, drop, seed, offset, st);
     double* part = reinterpret_cast<double*>(ws + p.partials_off);
     float* S1 = reinterpret_cast<float*>(ws + p.s1_off);
     float* S2 = reinterpret_cast<float*>(ws + p.s2_off);
@@ -1464,6 +1552,14 @@ int ptrb200_ffnet_backward(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* 
         }
     }
     return check_launch("ffnet_backward");
+}
+
+int ptrb200_ffnet_backward(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, const float* X,
+                           const float* dOut, float* dX, void* workspace, int64_t workspace_bytes,
+                           int B, int n, const int32_t* offsets, int total_rows, int training, uint64_t seed, uint64_t offset,
+                           ptrb200_stream_t stream) {
+    return ptrb200_ffnet_backward_x(net, grads, X, PTRB200_DTYPE_F32, dOut, dX, workspace, workspace_bytes, B, n, offsets,
+                                    total_rows, training, seed, offset, stream);
 }
 
 }  // extern "C"

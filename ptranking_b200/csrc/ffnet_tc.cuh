@@ -107,6 +107,21 @@ static __device__ __forceinline__ float4 ldg4_guard(const float* p, int k, int K
     return (k < K) ? __ldg(reinterpret_cast<const float4*>(p)) : make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
+// bf16 features (the layer-0 "XB" kernel variants): `base` holds bf16 values behind a float pointer.  Elements
+// elem .. elem+3 arrive in one 8-byte load (elem % 4 == 0, 8-byte aligned base: host guarantees) and widen exactly to fp32
+// -- a bf16 value is its fp32 value with the low 16 bits zero -- so everything downstream sees the same numbers an fp32
+// copy of the features would give.
+static __device__ __forceinline__ float4 ldg_bf16x4(const float* base, size_t elem) {
+    const uint2 u = __ldg(reinterpret_cast<const uint2*>(reinterpret_cast<const uint16_t*>(base) + elem));
+    return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xffff0000u),
+                       __uint_as_float(u.y << 16), __uint_as_float(u.y & 0xffff0000u));
+}
+template <bool XB>
+static __device__ __forceinline__ float4 ldg_a4(const float* base, size_t elem) {
+    if constexpr (XB) return ldg_bf16x4(base, elem);
+    else return __ldg(reinterpret_cast<const float4*>(base + elem));
+}
+
 // Builds the B-operand image of a [N,K] row-major matrix (TRANSPOSE=false) or of its transpose
 // (TRANSPOSE=true: image rows = columns of the source, used for dgrad's W^T): hi/lo tf32 split,
 // rows padded to NP, K cut into 128-byte chunks, each chunk [NP][128 B] in SWIZZLE_128B order.
@@ -183,7 +198,8 @@ __global__ void pack_b_image_kernel(const float* __restrict__ src, int src_rows,
 constexpr int RG_THREADS = 256;         // two warpgroups, 64 rows of the 128-row tile each
 constexpr int RG_MAX_N = 128;           // output columns per CTA: the accumulators of a 64 x 128 warpgroup tile fill 64 registers
 
-template <int MODE, int PASSES, int ACT = -1>
+// XB: g.P holds bf16 features (layer 0 only: FWD, no scale/shift, no activation)
+template <int MODE, int PASSES, int ACT = -1, bool XB = false>
 __global__ void __launch_bounds__(RG_THREADS) rows_gemm_tc_kernel(RowsGemmArgs g) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -243,7 +259,8 @@ __global__ void __launch_bounds__(RG_THREADS) rows_gemm_tc_kernel(RowsGemmArgs g
 #pragma unroll
         for (int i = 0; i < A_UNITS; ++i) {
             const int u = tid + i * RG_THREADS, r = u >> 3, j = u & 7, k = c * 32 + j * 4;
-            nav[i] = (r < nrows) ? ldg4_guard(g.P + (size_t)(row0 + r) * K + k, k, K) : make_float4(0.f, 0.f, 0.f, 0.f);
+            if constexpr (XB) nav[i] = (r < nrows && k < K) ? ldg_bf16x4(g.P, (size_t)(row0 + r) * K + k) : make_float4(0.f, 0.f, 0.f, 0.f);
+            else nav[i] = (r < nrows) ? ldg4_guard(g.P + (size_t)(row0 + r) * K + k, k, K) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
     };
     load_chunk(0);
@@ -406,7 +423,9 @@ static __device__ __forceinline__ void rw_tile(const RowsGemmArgs& g, int t, int
 //      on row / chunk address arithmetic, bounds predicates and the prefetch bookkeeping than on the prologue itself; with
 //      K known the chunk loops unroll completely and that arithmetic folds into immediates (instantiated for the widths
 //      of the default scorer, 136 and 100).
-template <int MODE, int PASSES, int ACT, int KT = 0>
+// XB:  g.P holds bf16 features (layer 0 only: FWD, no scale/shift, no activation); the producers load 4 of them as one
+//      8-byte unit and widen it before the unchanged prologue and split.
+template <int MODE, int PASSES, int ACT, int KT = 0, bool XB = false>
 __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArgs g, RowsWsExtra x) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -576,7 +595,7 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
                 if (partial && c == lastc) {
     #pragma unroll
                     for (int i = 0; i < RW_PU; ++i) {
-                        pre[i] = okB[i] ? __ldg(reinterpret_cast<const float4*>(g.P + soffB[i])) : make_float4(0.f, 0.f, 0.f, 0.f);
+                        pre[i] = okB[i] ? ldg_a4<XB>(g.P, soffB[i]) : make_float4(0.f, 0.f, 0.f, 0.f);
                         if (MODE == RG_DGRAD) pre2[i] = (fused_dz && okB[i]) ? __ldg(reinterpret_cast<const float4*>(g.P2 + soffB[i])) : make_float4(0.f, 0.f, 0.f, 0.f);
                     }
                     return;
@@ -584,7 +603,7 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
                 const bool kv = c * 32 + j4 < K;
     #pragma unroll
                 for (int i = 0; i < RW_PU; ++i) {
-                    pre[i] = (ok[i] && kv) ? __ldg(reinterpret_cast<const float4*>(g.P + soff[i] + c * 32)) : make_float4(0.f, 0.f, 0.f, 0.f);
+                    pre[i] = (ok[i] && kv) ? ldg_a4<XB>(g.P, soff[i] + c * 32) : make_float4(0.f, 0.f, 0.f, 0.f);
                     if (MODE == RG_DGRAD) pre2[i] = (fused_dz && ok[i] && kv) ? __ldg(reinterpret_cast<const float4*>(g.P2 + soff[i] + c * 32)) : make_float4(0.f, 0.f, 0.f, 0.f);
                 }
             };
@@ -849,7 +868,10 @@ constexpr int WG_MAX_STAGES = 4;      // raw-tile ring depth bound (TMA bulk cop
 // threads turn a raw tile into transposed hi/lo TF32 operand buffers (double buffered); the MMAs of a tile run
 // asynchronously while the next tile is staged.  Warpgroup w multiplies dZ columns [64 (w & 1), +64) by the input
 // columns of half (w >> 1) of the block.
-template <int PASSES>
+// XB: g.P holds bf16 features (layer 0).  The raw ring carries them at 2 bytes each and the staging widens them while
+// transposing.  A bulk copy needs 16-byte sizes and addresses; a P tile (or, column-blocked, a row segment) that does not
+// have them is copied by hand, as odd-sized dZ tiles are.
+template <int PASSES, bool XB = false>
 __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(WgradArgs g) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -864,7 +886,8 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(WgradArgs g) {
     const int op_bytes = (zop_bytes + pop_bytes) * (PASSES == 3 ? 2 : 1);
     const bool fused_dz = g.Z2 != nullptr;
     const int rawz1 = ((R * Nmax * 4 + 127) / 128) * 128;
-    const int rawz_bytes = rawz1 * (fused_dz ? 2 : 1), rawp_bytes = ((R * Kmax * 4 + 127) / 128) * 128;   // [dY | Z2] then the layer input
+    constexpr int PB = XB ? 2 : 4;                           // bytes per layer-input element in the raw ring
+    const int rawz_bytes = rawz1 * (fused_dz ? 2 : 1), rawp_bytes = ((R * Kmax * PB + 127) / 128) * 128;   // [dY | Z2] then the layer input
     const int stages = g.stages;
     unsigned char* opbuf = base;                             // [2][dZ hi | dZ lo | P hi | P lo]
     unsigned char* rawbuf = opbuf + 2 * op_bytes;            // [stages][rawz + rawp]
@@ -879,12 +902,21 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(WgradArgs g) {
     const int ntiles = (g.rows + R - 1) / R;
     const int my_tiles = blockIdx.x < ntiles ? (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
 
+    // bf16 layer input: can its tiles travel by bulk copy?  (fp32: always -- K % 4 == 0 and 16-byte aligned rows)
+    bool p_bulk_ok = true;
+    if constexpr (XB) p_bulk_ok = ((reinterpret_cast<uintptr_t>(g.P) & 15) == 0) && (!blocked || (K % 8 == 0 && g.K_full % 8 == 0));
+    auto p_bulk = [&](int nrows) -> bool {
+        if constexpr (XB) return p_bulk_ok && (blocked || (((uint32_t)nrows * K * 2) & 15) == 0);
+        else return true;
+    };
+
     // whole-warp call (warp 0): un-blocked tiles are contiguous in HBM (one copy per operand, issued by lane 0);
     // column blocks are row segments, one pair of copies per row, issued by lane = row
     auto issue_load = [&](int it, int s) {
         const int t = blockIdx.x + it * gridDim.x;
         const int row0 = t * R, nrows = min(R, g.rows - row0);
-        const uint32_t zb = (uint32_t)nrows * N * 4, pb = (uint32_t)nrows * K * 4;
+        const bool pbk = p_bulk(nrows);
+        const uint32_t zb = (uint32_t)nrows * N * 4, pb = pbk ? (uint32_t)nrows * K * PB : 0u;
         unsigned char* rz = rawbuf + s * (rawz_bytes + rawp_bytes);
         if (!blocked) {
             if (lane == 0) {
@@ -895,7 +927,8 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(WgradArgs g) {
                 } else {
                     tc::mbar_expect_tx(full + s, pb);     // odd-sized dZ tail tile: the threads copy it by hand
                 }
-                tc::bulk_g2s(rz + rawz_bytes, g.P + (size_t)row0 * K, pb, full + s);
+                if constexpr (XB) { if (pbk) tc::bulk_g2s(rz + rawz_bytes, reinterpret_cast<const uint16_t*>(g.P) + (size_t)row0 * K, pb, full + s); }
+                else tc::bulk_g2s(rz + rawz_bytes, g.P + (size_t)row0 * K, pb, full + s);
             }
         } else {
             const bool z_bulk = (N & 3) == 0;            // a dZ row segment must be a multiple of 16 bytes for TMA
@@ -903,7 +936,10 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(WgradArgs g) {
             __syncwarp();
             if (lane < nrows) {
                 if (z_bulk) tc::bulk_g2s(rz + (size_t)lane * N * 4, g.dZ + (size_t)(row0 + lane) * g.N_full + m0, (uint32_t)N * 4, full + s);
-                tc::bulk_g2s(rz + rawz_bytes + (size_t)lane * K * 4, g.P + (size_t)(row0 + lane) * g.K_full + kk0, (uint32_t)K * 4, full + s);
+                if constexpr (XB) {
+                    if (pbk) tc::bulk_g2s(rz + rawz_bytes + (size_t)lane * K * 2, reinterpret_cast<const uint16_t*>(g.P) + (size_t)(row0 + lane) * g.K_full + kk0,
+                                          (uint32_t)K * 2, full + s);
+                } else tc::bulk_g2s(rz + rawz_bytes + (size_t)lane * K * 4, g.P + (size_t)(row0 + lane) * g.K_full + kk0, (uint32_t)K * 4, full + s);
             }
             __syncwarp();
         }
@@ -959,6 +995,14 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(WgradArgs g) {
             for (int e = tid; e < nrows * N; e += WG_THREADS) rzw[e] = g.dZ[(size_t)(row0 + e / N) * g.N_full + m0 + e % N];
             __syncthreads();
         }
+        if constexpr (XB) {
+            if (!p_bulk(nrows)) {                            // bf16 layer input not TMA-sized or -aligned: copy by hand
+                uint16_t* rpw = reinterpret_cast<uint16_t*>(rawbuf + s * (rawz_bytes + rawp_bytes) + rawz_bytes);
+                const uint16_t* src = reinterpret_cast<const uint16_t*>(g.P);
+                for (int e = tid; e < nrows * K; e += WG_THREADS) rpw[e] = src[(size_t)(row0 + e / K) * g.K_full + kk0 + e % K];
+                __syncthreads();
+            }
+        }
         tc::mbar_wait(full + s, (it / stages) & 1);
         unsigned char* zh = opbuf + o * op_bytes;
         unsigned char* zl = zh + zop_bytes;
@@ -1001,7 +1045,8 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(WgradArgs g) {
                 const int r = qq * 4 + e;
                 float x = 0.0f;
                 if (r < nrows) {
-                    x = rp[r * K + k];
+                    if constexpr (XB) x = __uint_as_float((uint32_t)reinterpret_cast<const uint16_t*>(rp)[r * K + k] << 16);
+                    else x = rp[r * K + k];
                     if (!plain_p) {
                         const int row = row0 + r, col = kk0 + k;
                         if (g.scale) {

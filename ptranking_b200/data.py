@@ -26,6 +26,24 @@ def presort_query(features: np.ndarray, labels: np.ndarray) -> Tuple[np.ndarray,
     return features[order], labels[order]
 
 
+def _check_feature_dtype(dtype: torch.dtype) -> torch.dtype:
+    if dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError(f"feature_dtype must be torch.float32 or torch.bfloat16, got {dtype}")
+    return dtype
+
+
+def features_to(X: np.ndarray, dtype: torch.dtype):
+    """One query's fp32 features as the loaders keep them: the numpy array itself for torch.float32; for torch.bfloat16 a
+    bf16 tensor, converted once here (round to nearest even).  bf16 batches halve the pinned host memory and the
+    host-to-device copy, and the scorer's layer-0 kernels read them natively, with the results the same values give in
+    fp32.  Pass features that are already scaled: raw LETOR features lose precision in bf16."""
+    return X if dtype == torch.float32 else torch.from_numpy(X).to(dtype)
+
+
+def _as_tensor(Xq) -> torch.Tensor:
+    return Xq if isinstance(Xq, torch.Tensor) else torch.from_numpy(Xq)
+
+
 class LengthBucketedBatches:
     """Iterable of ``(qids, X[B,n,F], y[B,n])`` CPU batches (pinned when CUDA is available).
 
@@ -36,13 +54,16 @@ class LengthBucketedBatches:
     drop_ragged     : drop the last, smaller batch of each length instead of emitting it
     rank / world    : data-parallel sharding -- every rank walks the same batch list and keeps batches rank::world,
                       so all ranks see the same number of batches per epoch (the last ``len % world`` are dropped)
+    feature_dtype   : torch.float32 (default) or torch.bfloat16 -- see :func:`features_to`
     """
 
     def __init__(self, queries: Iterable[Query], docs_per_batch: int = 1 << 18, max_queries: Optional[int] = None,
                  presort: bool = True, shuffle_seed: Optional[int] = None, drop_ragged: bool = False,
-                 rank: int = 0, world: int = 1, pin_memory: Optional[bool] = None):
+                 rank: int = 0, world: int = 1, pin_memory: Optional[bool] = None,
+                 feature_dtype: torch.dtype = torch.float32):
         if docs_per_batch < 1 or world < 1 or not (0 <= rank < world):
             raise ValueError("docs_per_batch >= 1 and 0 <= rank < world are required")
+        self.feature_dtype = _check_feature_dtype(feature_dtype)
         self.docs_per_batch, self.max_queries = int(docs_per_batch), max_queries
         self.shuffle_seed, self.drop_ragged, self.rank, self.world = shuffle_seed, drop_ragged, rank, world
         self.pin = torch.cuda.is_available() if pin_memory is None else bool(pin_memory)
@@ -62,7 +83,7 @@ class LengthBucketedBatches:
                 raise ValueError(f"query {qid}: {X.shape[1]} features, expected {self.num_features}")
             if presort:
                 X, y = presort_query(X, y)
-            self.buckets[X.shape[0]].append((str(qid), X, y))
+            self.buckets[X.shape[0]].append((str(qid), features_to(X, self.feature_dtype), y))
 
     def batch_size(self, n: int) -> int:
         B = max(1, self.docs_per_batch // n)
@@ -94,10 +115,10 @@ class LengthBucketedBatches:
         self.epoch += 1
         for n, members in plan:
             qs = [self.buckets[n][i] for i in members]
-            X = torch.empty((len(qs), n, self.num_features), dtype=torch.float32, pin_memory=self.pin)
+            X = torch.empty((len(qs), n, self.num_features), dtype=self.feature_dtype, pin_memory=self.pin)
             y = torch.empty((len(qs), n), dtype=torch.float32, pin_memory=self.pin)
             for b, (_, Xq, yq) in enumerate(qs):
-                X[b] = torch.from_numpy(Xq)
+                X[b] = _as_tensor(Xq)
                 y[b] = torch.from_numpy(yq)
             yield [q[0] for q in qs], X, y
 
@@ -151,12 +172,15 @@ class RaggedBatches:
 
     def __init__(self, queries: Iterable[Query], docs_per_batch: int = 1 << 18, max_queries: Optional[int] = None,
                  presort: bool = True, shuffle_seed: Optional[int] = None, rank: int = 0, world: int = 1,
-                 pin_memory: Optional[bool] = None, max_list_len: int = 4096, bucket_edges: Sequence[int] = (128, 512)):
+                 pin_memory: Optional[bool] = None, max_list_len: int = 4096, bucket_edges: Sequence[int] = (128, 512),
+                 feature_dtype: torch.dtype = torch.float32):
         """``bucket_edges``: upper ends of the length classes a batch is cut into (:func:`length_buckets`).  The default
         suits the pairwise-loss kernels; the list scorer pads every class to its longest list and attention work grows
-        with the square of that length, so it is better served by finer classes, e.g. (32, 64, 128, 256)."""
+        with the square of that length, so it is better served by finer classes, e.g. (32, 64, 128, 256).
+        ``feature_dtype``: torch.float32 (default) or torch.bfloat16 -- see :func:`features_to`."""
         if docs_per_batch < 1 or world < 1 or not (0 <= rank < world):
             raise ValueError("docs_per_batch >= 1 and 0 <= rank < world are required")
+        self.feature_dtype = _check_feature_dtype(feature_dtype)
         if list(bucket_edges) != sorted(set(int(e) for e in bucket_edges)) or any(int(e) < 1 for e in bucket_edges):
             raise ValueError("bucket_edges must be increasing positive lengths")
         self.bucket_edges = tuple(int(e) for e in bucket_edges)
@@ -181,7 +205,7 @@ class RaggedBatches:
                 raise ValueError(f"query {qid}: {X.shape[1]} features, expected {self.num_features}")
             if presort:
                 X, y = presort_query(X, y)
-            self.queries.append((str(qid), X, y))
+            self.queries.append((str(qid), features_to(X, self.feature_dtype), y))
 
     def _plan(self) -> List[List[int]]:
         idx = np.arange(len(self.queries))
@@ -210,13 +234,13 @@ class RaggedBatches:
             qs = sorted((self.queries[i] for i in members), key=lambda q: -q[1].shape[0])
             lens = np.array([q[1].shape[0] for q in qs], dtype=np.int64)
             total = int(lens.sum())
-            X = torch.empty((total, self.num_features), dtype=torch.float32, pin_memory=self.pin)
+            X = torch.empty((total, self.num_features), dtype=self.feature_dtype, pin_memory=self.pin)
             y = torch.empty((total,), dtype=torch.float32, pin_memory=self.pin)
             offsets = torch.zeros(len(qs) + 1, dtype=torch.int32, pin_memory=self.pin)
             offsets[1:] = torch.from_numpy(np.cumsum(lens)).to(torch.int32)
             o = 0
             for _, Xq, yq in qs:
-                X[o: o + Xq.shape[0]] = torch.from_numpy(Xq)
+                X[o: o + Xq.shape[0]] = _as_tensor(Xq)
                 y[o: o + Xq.shape[0]] = torch.from_numpy(yq)
                 o += Xq.shape[0]
             yield [q[0] for q in qs], X, y, offsets, int(lens.max()), length_buckets(lens, edges=self.bucket_edges)

@@ -49,6 +49,14 @@ def _dev_f32(t: torch.Tensor, name: str) -> torch.Tensor:
     return t.contiguous()
 
 
+def _dev_features(t: torch.Tensor, name: str):
+    """-> (contiguous CUDA tensor, PTRB200_DTYPE_* code).  bf16 features pass through as they are (the scorer's layer-0
+    kernels read them natively); every other dtype is upcast to fp32 as by :func:`_dev_f32`."""
+    if t.is_cuda and t.dtype == torch.bfloat16:
+        return t.contiguous(), _lib.DTYPE_BF16
+    return _dev_f32(t, name), _lib.DTYPE_F32
+
+
 def _list_layout(s: torch.Tensor, offsets, max_len):
     """-> (B, n, offsets tensor or None, offsets pointer or None).  Dense batches: ``s`` is [B,n] and offsets is None.
     Ragged batches (SURVEY 8f-2): ``s`` is the flat [total_docs] array, ``offsets`` the int32 [B+1] prefix offsets on the
@@ -384,9 +392,15 @@ def shuffle_ties_perm(labels: torch.Tensor, seed: Optional[int] = None, offset: 
 # --------------------------------------------------------------------------- #
 @_on_tensor_device
 def standard_scale(X: torch.Tensor, offsets: Optional[torch.Tensor] = None, max_len: Optional[int] = None,
-                   clip_max: Optional[float] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+                   clip_max: Optional[float] = None, out: Optional[torch.Tensor] = None,
+                   out_dtype: torch.dtype = torch.float32) -> torch.Tensor:
     """Per-query StandardScaler (data_utils.py:482-487) on the device.  X: [B,n,F], or flat [total_docs,F] with
-    ``offsets``/``max_len``.  ``clip_max``: clamp features first (the loader's ISTELLA_MAX clip)."""
+    ``offsets``/``max_len``.  ``clip_max``: clamp features first (the loader's ISTELLA_MAX clip).
+    ``out_dtype=torch.bfloat16``: the fp32 result rounded to nearest even at the store -- equal to
+    ``standard_scale(...).to(torch.bfloat16)`` without the fp32 intermediate (scaling comes first: raw features lose
+    precision in bf16).  Not in place."""
+    if out_dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError(f"out_dtype must be torch.float32 or torch.bfloat16, got {out_dtype}")
     lib = _lib.load()
     X = _dev_f32(X, "X")
     if offsets is None:
@@ -399,9 +413,17 @@ def standard_scale(X: torch.Tensor, offsets: Optional[torch.Tensor] = None, max_
         offsets = offsets.to(device=X.device, dtype=torch.int32).contiguous()
         B, n, F, op = offsets.numel() - 1, max(int(max_len), 1), X.shape[1], offsets.data_ptr()
     if out is None:
-        out = torch.empty_like(X)
-    _lib.check(lib.ptrb200_standard_scale(X.data_ptr(), op, out.data_ptr(), B, n, F, int(clip_max is not None),
-                                          float(clip_max if clip_max is not None else 0.0), _stream_ptr()), "standard_scale")
+        out = torch.empty_like(X, dtype=out_dtype)
+    elif out_dtype == torch.bfloat16 and (out.dtype != out_dtype or out.shape != X.shape or not out.is_contiguous()
+                                          or out.device != X.device):
+        raise ValueError(f"out must be a contiguous {out_dtype} tensor of shape {tuple(X.shape)} on {X.device}")
+    clip, cmax = int(clip_max is not None), float(clip_max if clip_max is not None else 0.0)
+    if out_dtype == torch.bfloat16:
+        _lib.check(lib.ptrb200_standard_scale_bf16(X.data_ptr(), op, out.data_ptr(), B, n, F, clip, cmax, _stream_ptr()),
+                   "standard_scale_bf16")
+    else:
+        _lib.check(lib.ptrb200_standard_scale(X.data_ptr(), op, out.data_ptr(), B, n, F, clip, cmax, _stream_ptr()),
+                   "standard_scale")
     return out
 
 
@@ -542,7 +564,7 @@ class _FFNetFn(torch.autograd.Function):
     @_on_tensor_device
     def forward(ctx, X, spec: FFNetSpec, training: bool, seed: int, offset: int, grad_targets, need_backward, ragged, *params):
         lib = _lib.load()
-        X = _dev_f32(X, "X")
+        X, x_dtype = _dev_features(X, "X")        # bf16 stays bf16: no fp32 copy of the features
         if ragged is None:          # dense [B,n,F]
             B, n, F = X.shape
             offsets, op, total = None, None, 0
@@ -557,7 +579,7 @@ class _FFNetFn(torch.autograd.Function):
             raise ValueError(f"feature width {F} != net input width {spec.dims[0]}")
         params = [p.detach().contiguous() for p in params]
         desc = spec.describe(params)
-        nbytes = lib.ptrb200_ffnet_workspace_bytes(C.byref(desc), B, n, total)
+        nbytes = lib.ptrb200_ffnet_workspace_bytes_x(C.byref(desc), x_dtype, B, n, total)
         if nbytes < 0:
             _lib.check(int(nbytes), "ffnet_workspace_bytes")
         ws = torch.empty(int(nbytes), dtype=torch.uint8, device=X.device)
@@ -566,9 +588,10 @@ class _FFNetFn(torch.autograd.Function):
         # caller runs under torch.no_grad()), so the by-products the backward pass reads are not written
         flags = int(training) | (0 if need_backward else 2)
         with _b200dist().call_context(ws, None):
-            _lib.check(lib.ptrb200_ffnet_forward(C.byref(desc), X.data_ptr(), out.data_ptr(), ws.data_ptr(), int(nbytes),
-                                                 B, n, op, total, flags, seed, offset, _stream_ptr()), "ffnet_forward")
-        ctx.spec, ctx.training, ctx.seed, ctx.offset = spec, training, seed, offset
+            _lib.check(lib.ptrb200_ffnet_forward_x(C.byref(desc), X.data_ptr(), x_dtype, out.data_ptr(), ws.data_ptr(),
+                                                   int(nbytes), B, n, op, total, flags, seed, offset, _stream_ptr()),
+                       "ffnet_forward")
+        ctx.spec, ctx.training, ctx.seed, ctx.offset, ctx.x_dtype = spec, training, seed, offset, x_dtype
         ctx.shape = (B, n, offsets, total)
         ctx.grad_targets = grad_targets
         ctx.ws, ctx.nbytes = (ws if need_backward else None), int(nbytes)
@@ -586,7 +609,8 @@ class _FFNetFn(torch.autograd.Function):
         desc = spec.describe(params)
         gdesc, gouts = spec.grads(params, ctx.grad_targets)
         d_out = _dev_f32(d_out, "d_out")
-        dX = torch.empty_like(X) if ctx.need_dx else None
+        # dX is computed in fp32 whatever X's dtype; autograd casts it to X's dtype on the way out
+        dX = torch.empty(X.shape, dtype=torch.float32, device=X.device) if ctx.need_dx else None
         # per-layer gradient tensors (write-through targets only): lets a data-parallel bucket start reducing a layer's
         # slice as soon as the library reports it complete
         layer_targets = None
@@ -596,10 +620,10 @@ class _FFNetFn(torch.autograd.Function):
                 layer_targets.append(gouts[i: i + len(names)])
                 i += len(names)
         with _b200dist().call_context(ctx.ws, layer_targets):
-            _lib.check(lib.ptrb200_ffnet_backward(C.byref(desc), C.byref(gdesc), X.data_ptr(), d_out.data_ptr(),
-                                                  dX.data_ptr() if dX is not None else None, ctx.ws.data_ptr(), ctx.nbytes,
-                                                  B, n, offsets.data_ptr() if offsets is not None else None, total,
-                                                  int(ctx.training), ctx.seed, ctx.offset, _stream_ptr()),
+            _lib.check(lib.ptrb200_ffnet_backward_x(C.byref(desc), C.byref(gdesc), X.data_ptr(), ctx.x_dtype, d_out.data_ptr(),
+                                                    dX.data_ptr() if dX is not None else None, ctx.ws.data_ptr(), ctx.nbytes,
+                                                    B, n, offsets.data_ptr() if offsets is not None else None, total,
+                                                    int(ctx.training), ctx.seed, ctx.offset, _stream_ptr()),
                        "ffnet_backward")
         ctx.ws = None
         if ctx.grad_targets is not None:            # written straight into the parameters' .grad storage
