@@ -152,6 +152,21 @@ int ptrb200_wassrank_fwd_bwd(const float* scores, const float* labels, const int
                              float* loss_per_query, int B, int n, int batch_queries, int cost_type, float lam,
                              int sh_itr, float non_rele_gap, float var_penalty, float gain_base, ptrb200_stream_t stream);
 
+/* MDPRank.custom_loss_function, ptranking/ltr_adhoc/listwise/mdprank.py:24-79 (+ sample_ranking_PL /
+ * sample_ranking_PL_gumbel_softmax, ltr_adhoc/util/sampling_utils.py:31-79).  One sampled ranking per query at any B;
+ * loss_per_query[b] is the query's REINFORCE loss (their sum is the reference's batch loss).  The ranking is drawn by
+ * sorting Gumbel-perturbed keys, s/T + g (PL) or (s + g)/T (STPL), g from `unif` (optional, same layout as scores) or
+ * from Philox4x32-10 keyed by (seed, offset, doc).  perm (optional, PL only): the ordering itself, as positions within
+ * each query's list.  sample_out (optional): receives the ordering used.  top_k <= 0 means the whole list; top_k beyond
+ * a list's length is clamped to it. */
+#define PTRB200_MDP_PL   0
+#define PTRB200_MDP_STPL 1
+int ptrb200_mdprank_fwd_bwd(const float* scores, const float* labels, const int32_t* offsets,
+                            const int32_t* perm, const float* unif, int32_t* sample_out,
+                            float* grad, float* loss_per_query, int B, int n, int top_k, float gamma,
+                            float temperature, int distribution, uint64_t seed, uint64_t offset,
+                            ptrb200_stream_t stream);
+
 /* deterministic (fixed-order) sum of n floats into out[0] -- the `torch.sum` over queries
  * that ends every reference loss (e.g. lambdarank.py:56). */
 int ptrb200_sum_f32(const float* x, float* out, int n, ptrb200_stream_t stream);

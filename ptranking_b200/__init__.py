@@ -18,10 +18,11 @@ from .ltr_adhoc.listwise.rank_cosine import RankCosine
 from .ltr_adhoc.listwise.st_listnet import STListNet
 from .ltr_adhoc.listwise.softrank import SoftRank
 from .ltr_adhoc.listwise.wassrank import WassRank
+from .ltr_adhoc.listwise.mdprank import MDPRank
 from .base.ranker import LABEL_TYPE
 
 MODELS = {c.__name__: c for c in (RankNet, LambdaRank, LambdaLoss, ListNet, ListMLE, ApproxNDCG,
-                                  RankMSE, RankCosine, STListNet, SoftRank, WassRank)}
+                                  RankMSE, RankCosine, STListNet, SoftRank, WassRank, MDPRank)}
 __version__ = "0.1.0"
 
 
@@ -34,4 +35,14 @@ def install(module=None):
     for name, cls in MODELS.items():
         previous[name] = getattr(module, name, None)
         setattr(module, name, cls)
+    # The driver also looks up globals()[model_id + "Parameter"] (ltr.py:463), and the reference's ltr.py imports no
+    # MDPRankParameter: supply the reference's own class, when its module is importable.
+    if getattr(module, 'MDPRankParameter', None) is None:
+        try:
+            from ptranking.ltr_adhoc.listwise.mdprank import MDPRankParameter
+        except ImportError:
+            pass
+        else:
+            previous['MDPRankParameter'] = getattr(module, 'MDPRankParameter', None)
+            setattr(module, 'MDPRankParameter', MDPRankParameter)
     return previous

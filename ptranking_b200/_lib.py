@@ -20,6 +20,7 @@ NORM_CODES = {None: 0, "BN": 1, "BN2": 2}
 MATH_MODES = {"simt": 0, "3xtf32": 1, "tf32": 2, "bf16": 3}
 LAMBDALOSS_TYPES = {"NDCG_Loss1": 0, "NDCG_Loss2": 1, "NDCG_Loss2++": 2}
 WASS_COST_TYPES = {"p1": 0, "p2": 1, "eg": 2, "dg": 3, "ddg": 4}   # PTRB200_WASS_COST_*
+MDP_DISTRIBUTIONS = {"PL": 0, "STPL": 1}                            # PTRB200_MDP_*
 DTYPE_F32, DTYPE_BF16 = 0, 1                                       # PTRB200_DTYPE_*: feature element type of the _x entries
 
 _fp = C.c_void_p   # device pointers travel as integers
@@ -73,6 +74,7 @@ SIGNATURES = {
     "ptrb200_softrank_fwd_bwd": (_I, [_fp, _fp, _fp, _fp, _fp, _I, _I, _F, _I, _fp]),
     "ptrb200_sinkstep": (_I, [_fp, _fp, _fp, _fp, _I, _I, _I, _F, _fp]),
     "ptrb200_wassrank_fwd_bwd": (_I, [_fp, _fp, _fp, _fp, _fp, _I, _I, _I, _I, _F, _I, _F, _F, _F, _fp]),
+    "ptrb200_mdprank_fwd_bwd": (_I, [_fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _I, _I, _I, _F, _F, _I, _U64, _U64, _fp]),
     "ptrb200_standard_scale": (_I, [_fp, _fp, _fp, _I, _I, _I, _I, _F, _fp]),
     "ptrb200_sum_f32": (_I, [_fp, _fp, _I, _fp]),
     "ptrb200_ndcg_at_ks": (_I, [_fp, _fp, _fp, C.POINTER(C.c_int32), _I, _fp, _fp, _I, _I, _I, _fp]),

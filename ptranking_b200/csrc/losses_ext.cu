@@ -6,6 +6,7 @@
 //   RankCosine  ptranking/ltr_adhoc/listwise/rank_cosine.py:33 (nn.CosineSimilarity(dim=1), eps 1e-8)
 //   STListNet   ptranking/ltr_adhoc/listwise/st_listnet.py:41-49
 //   SoftRank    ptranking/ltr_adhoc/listwise/softrank.py:46-72
+//   MDPRank     ptranking/ltr_adhoc/listwise/mdprank.py:24-79 (+ sample_ranking_PL / _gumbel_softmax, util/sampling_utils.py:31-79)
 //   sinkstep    ptranking/ltr_adhoc/listwise/wassrank/pytorch_wasserstein.py:132-224 (CUDA string) / :277-291 (CPU form)
 #include "losses_common.cuh"
 
@@ -154,6 +155,142 @@ __global__ void softrank_kernel(const float* __restrict__ scores, const float* _
 }
 
 // ---------------------------------------------------------------------------
+// MDPRank: REINFORCE on one sampled Plackett-Luce ranking sigma per query (mdprank.py:24-79).
+// Sampling is Gumbel-top-k: sort keys s/T + g (PL) or (s + g)/T (STPL), g from the uniforms as in stlistnet_kernel;
+// an injected PL ordering `perm` replaces the sort.  Action values a_t = s_sigma(t) (PL) or the perturbed key (STPL).
+// Returns G_t = gamma^{t+1} sum_{t<=t'<k} (2^y_sigma(t') - 1) / log2(t'+2), C_t = sum_{j>=t} exp(a_j) over the whole
+// list; loss = sum_{t<k} (log C_t - a_t) G_t, d loss / d a_j = sum_{t<=min(j,k-1)} G_t exp(a_j - log C_t) - [j<k] G_j,
+// scattered to s_sigma(j) (times 1/T under STPL, where a depends on s through the division).
+// Both sums over t are scans of (shift, sum) pairs, so nothing overflows or underflows where the action values spread
+// over more than fp32's exponent range (STPL at small T): log C_t is exact to rounding at every position, and for STPL,
+// whose a_t descend, log C_t - a_t is the log of a sum of terms <= 1 with no cancellation.
+// ---------------------------------------------------------------------------
+// (m, s) <- (m, s) + (m2, s2) for the value s e^m; m = -inf with s = 0 is the empty sum.
+static __device__ __forceinline__ void lse_add(float& m, float& s, float m2, float s2) {
+    if (m2 > m) { s = s * expf(m - m2) + s2; m = m2; }
+    else if (m2 > -INFINITY) s += s2 * expf(m2 - m);
+}
+
+// Inclusive scan of pairs (mx[i], sm[i]) under lse_add, forward or reverse; the schedule of block_scan_inclusive.
+template <bool REVERSE>
+static __device__ void block_scan_lse(float* mx, float* sm, int n, float* red /* >= 128 floats */) {
+    const int T = blockDim.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = (T + 31) >> 5;
+    const int C = (n + T - 1) / T;
+    const int c0 = min(tid * C, n), c1 = min(c0 + C, n);
+    float rm = -INFINITY, rs = 0.0f;
+    for (int i = c0; i < c1; ++i) {
+        const int p = REVERSE ? n - 1 - i : i;
+        lse_add(rm, rs, mx[p], sm[p]);
+        mx[p] = rm; sm[p] = rs;
+    }
+    float im = rm, is = rs;                              // inclusive over the lanes of the warp
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const float tm = __shfl_up_sync(0xffffffffu, im, o), ts = __shfl_up_sync(0xffffffffu, is, o);
+        if (lane >= o) lse_add(im, is, tm, ts);
+    }
+    float em = __shfl_up_sync(0xffffffffu, im, 1), es = __shfl_up_sync(0xffffffffu, is, 1);
+    if (lane == 0) { em = -INFINITY; es = 0.0f; }
+    __syncthreads();
+    if (lane == 31) { red[warp] = im; red[32 + warp] = is; }
+    __syncthreads();
+    if (warp == 0) {
+        float wm = lane < nw ? red[lane] : -INFINITY, ws = lane < nw ? red[32 + lane] : 0.0f;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const float tm = __shfl_up_sync(0xffffffffu, wm, o), ts = __shfl_up_sync(0xffffffffu, ws, o);
+            if (lane >= o) lse_add(wm, ws, tm, ts);
+        }
+        float xm = __shfl_up_sync(0xffffffffu, wm, 1), xs = __shfl_up_sync(0xffffffffu, ws, 1);
+        if (lane == 0) { xm = -INFINITY; xs = 0.0f; }
+        red[64 + lane] = xm; red[96 + lane] = xs;       // exclusive over warps
+    }
+    __syncthreads();
+    lse_add(em, es, red[64 + warp], red[96 + warp]);
+    if (em > -INFINITY) {
+        for (int i = c0; i < c1; ++i) {
+            const int p = REVERSE ? n - 1 - i : i;
+            float m = mx[p], s = sm[p];
+            lse_add(m, s, em, es);
+            mx[p] = m; sm[p] = s;
+        }
+    }
+    __syncthreads();
+}
+
+__global__ void mdprank_kernel(const float* __restrict__ scores, const float* __restrict__ labels, const int32_t* __restrict__ offsets,
+                               const int32_t* __restrict__ perm, const float* __restrict__ unif, int32_t* __restrict__ sample_out,
+                               float* __restrict__ grad, float* __restrict__ loss_q, int nmax, int npow2max, int top_k,
+                               float gamma, float temperature, int stpl, uint64_t seed, uint64_t offset) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    u64* keys = reinterpret_cast<u64*>(smem_raw);
+    float* v = reinterpret_cast<float*>(keys + npow2max);     // by document: the value a takes when the document is drawn
+    int* pid = reinterpret_cast<int*>(v + nmax);              // by position: sigma
+    float* lm = reinterpret_cast<float*>(pid + nmax);         // by position: (shift, sum) pairs of C_t, then of
+    float* ls = lm + nmax;                                    //   sum_{t'<=t} G_t' / C_t'
+    float* G = ls + nmax;                                     // rewards, then returns (first k positions)
+    float* red = G + nmax;
+    const int b = blockIdx.x;
+    const ListSpan sp = list_span(offsets, b, nmax);
+    const int n = sp.n, npow2 = offsets ? next_pow2(n) : npow2max;
+    if (n == 0) { if (threadIdx.x == 0) loss_q[b] = 0.0f; return; }
+    const int k = (top_k > 0 && top_k < n) ? top_k : n;
+    if (perm) {
+        for (int i = threadIdx.x; i < n; i += blockDim.x) {
+            pid[i] = clampi(perm[sp.base + i], 0, n - 1);      // positions within the query's own list
+            v[i] = scores[sp.base + i];
+        }
+    } else {
+        for (int i = threadIdx.x; i < npow2; i += blockDim.x) {
+            u64 key = 0ull;
+            if (i < n) {
+                float u;
+                if (unif) u = unif[sp.base + i];
+                else u = (float)(dropout_bits(seed, offset, (uint64_t)(sp.base + i)) >> 8) * (1.0f / 16777216.0f);
+                const float g = -logf(-logf(u + 1e-20f) + 1e-20f);
+                const float s = scores[sp.base + i];
+                const float z = stpl ? __fdiv_rn(s + g, temperature) : __fdiv_rn(s, temperature) + g;
+                v[i] = stpl ? z : s;
+                key = desc_key(z, i);
+            }
+            keys[i] = key;
+        }
+        block_sort_desc(keys, npow2);
+        for (int t = threadIdx.x; t < n; t += blockDim.x) pid[t] = key_index(keys[t]);
+    }
+    __syncthreads();
+    for (int t = threadIdx.x; t < n; t += blockDim.x) {
+        const int id = pid[t];
+        lm[t] = v[id]; ls[t] = 1.0f;
+        if (t < k) G[t] = gain_of(labels[sp.base + id]) / log2_rank(t);
+        if (sample_out) sample_out[sp.base + t] = id;
+    }
+    __syncthreads();
+    block_scan_lse<true>(lm, ls, n, red);                // C_t = ls e^lm
+    block_scan_inclusive<true>(G, k, red);               // returns within the top-k window
+    float loss = 0.0f;
+    for (int t = threadIdx.x; t < k; t += blockDim.x) {
+        float Gt = G[t];
+        if (gamma != 1.0f) { Gt *= powf(gamma, (float)(t + 1)); G[t] = Gt; }   // mdprank.py:59-61, applied after the sum
+        const float lc = lm[t] + logf(ls[t]);
+        loss += ((lm[t] - v[pid[t]]) + logf(ls[t])) * Gt;
+        lm[t] = Gt != 0.0f ? logf(fabsf(Gt)) - lc : -INFINITY;                    // G_t / C_t = ls e^lm
+        ls[t] = Gt > 0.0f ? 1.0f : (Gt < 0.0f ? -1.0f : 0.0f);
+    }
+    __syncthreads();
+    block_scan_lse<false>(lm, ls, k, red);               // Q_t = sum_{t'<=t} G_t' / C_t'
+    const float qm = lm[k - 1], qs = ls[k - 1];
+    for (int j = threadIdx.x; j < n; j += blockDim.x) {
+        const float a = v[pid[j]];
+        float gj = j < k ? ls[j] * expf(a + lm[j]) - G[j] : qs * expf(a + qm);
+        if (stpl) gj = __fdiv_rn(gj, temperature);
+        grad[sp.base + pid[j]] = gj;
+    }
+    loss = block_sum(loss, red);
+    if (threadIdx.x == 0) loss_q[b] = loss;
+}
+
+// ---------------------------------------------------------------------------
 // Sinkhorn half-step:  log_v[b][j] = log_nu[b][j] - logsumexp_i( -dist[i][j] / lambda + log_u[b][i] ).
 // One CTA per (tile of 32 columns j, b): lane = column (coalesced reads of dist rows), the 8 warps split the reduction
 // rows i, each lane keeps an online (max, sum-exp) pair, the eight partials of a column are merged through shared
@@ -236,6 +373,29 @@ int ptrb200_softrank_fwd_bwd(const float* scores, const float* labels, const int
     if ((rc = allow_smem(softrank_kernel, smem))) return rc;
     PTRB200_LAUNCH(softrank_kernel, B, block_threads(n), smem, stream, scores, labels, offsets, grad, loss_per_query, n, 1.0f / den, top_k);
     return check_launch("softrank");
+}
+
+int ptrb200_mdprank_fwd_bwd(const float* scores, const float* labels, const int32_t* offsets, const int32_t* perm,
+                            const float* unif, int32_t* sample_out, float* grad, float* loss_per_query, int B, int n,
+                            int top_k, float gamma, float temperature, int distribution, uint64_t seed, uint64_t offset,
+                            ptrb200_stream_t stream) {
+    int rc = check_list_args(scores, labels, grad, loss_per_query, B, n);
+    if (rc) return rc;
+    if (distribution != PTRB200_MDP_PL && distribution != PTRB200_MDP_STPL) {
+        set_error("mdprank: unknown distribution %d", distribution);
+        return PTRB200_ERR_INVALID;
+    }
+    if (!(temperature > 0.0f)) { set_error("mdprank: temperature must be positive"); return PTRB200_ERR_INVALID; }
+    if (perm && distribution == PTRB200_MDP_STPL) {
+        set_error("mdprank: an injected ordering is PL only (STPL's action values come from the uniforms)");
+        return PTRB200_ERR_INVALID;
+    }
+    const int npow2 = next_pow2(n);
+    const size_t smem = (size_t)npow2 * 8 + (size_t)n * 4 * 5 + 128 * 4;
+    if ((rc = allow_smem(mdprank_kernel, smem))) return rc;
+    PTRB200_LAUNCH(mdprank_kernel, B, block_threads(n), smem, stream, scores, labels, offsets, perm, unif, sample_out, grad,
+                   loss_per_query, n, npow2, top_k, gamma, temperature, distribution == PTRB200_MDP_STPL ? 1 : 0, seed, offset);
+    return check_launch("mdprank");
 }
 
 int ptrb200_sinkstep(const float* dist, const float* log_nu, const float* log_u, float* log_v,

@@ -128,7 +128,7 @@ def _loss_call(name: str, scores: torch.Tensor, labels: torch.Tensor, params: di
         aux = y
     yp = aux.data_ptr()
     unif = None
-    if name == "STListNet":
+    if name in ("STListNet", "MDPRank"):
         unif = params.get("unif")
         if unif is not None:
             unif = _dev_f32(unif, "unif")
@@ -139,6 +139,18 @@ def _loss_call(name: str, scores: torch.Tensor, labels: torch.Tensor, params: di
             seed = torch.initial_seed()
         if offset is None:
             offset = next_noise_offset()
+    if name == "MDPRank":
+        dist = params.get("distribution", "PL")
+        if dist not in _lib.MDP_DISTRIBUTIONS:
+            raise ValueError(f"MDPRank distribution must be one of {sorted(_lib.MDP_DISTRIBUTIONS)}, got {dist!r}")
+        mdp_perm, sample_out = params.get("perm"), params.get("sample_out")
+        if mdp_perm is not None:
+            mdp_perm = mdp_perm.to(device=s.device, dtype=torch.int32).contiguous()
+            if mdp_perm.shape != s.shape:
+                raise ValueError(f"perm {tuple(mdp_perm.shape)} does not match scores {tuple(s.shape)}")
+        if sample_out is not None and not (sample_out.device == s.device and sample_out.dtype == torch.int32
+                                           and sample_out.is_contiguous() and sample_out.shape == s.shape):
+            raise ValueError("sample_out must be a contiguous int32 tensor of the scores' shape on their device")
     # ApproxNDCG scratch: Bq + 1 floats per launch; concurrent buckets get disjoint pieces
     scratch = torch.empty(B + len(ranges), dtype=torch.float32, device=s.device) if name == "ApproxNDCG" else None
     # The first bucket holds the longest lists: few CTAs that run long.  It goes onto a side stream so that the short-list
@@ -184,6 +196,14 @@ def _loss_call(name: str, scores: torch.Tensor, labels: torch.Tensor, params: di
             rc = lib.ptrb200_wassrank_fwd_bwd(sp, yp, opq, gp, lqq, Bq, nq, B, _lib.WASS_COST_TYPES[cost], float(params.get("lam", 0.1)),
                                               int(params.get("sh_itr", 20)), float(params.get("non_rele_gap", 100.0)),
                                               float(params.get("var_penalty", math.e)), float(params.get("gain_base", 4.0)), st)
+        elif name == "MDPRank":
+            top_k = params.get("top_k")
+            rc = lib.ptrb200_mdprank_fwd_bwd(sp, yp, opq, None if mdp_perm is None else mdp_perm.data_ptr(),
+                                             None if unif is None else unif.data_ptr(),
+                                             None if sample_out is None else sample_out.data_ptr(), gp, lqq, Bq, nq,
+                                             int(top_k) if top_k else 0, float(params.get("gamma", 1.0)),
+                                             float(params.get("temperature", 1.0)), _lib.MDP_DISTRIBUTIONS[dist],
+                                             seed & (2 ** 64 - 1), offset & (2 ** 64 - 1), st)
         else:
             raise NotImplementedError(name)
         _lib.check(rc, f"{name} loss kernel")
@@ -206,7 +226,7 @@ _noise_offset = 0
 
 
 def next_noise_offset() -> int:
-    """Counter that keys the Gumbel draw of successive STListNet calls (same role as the tie-shuffle counter)."""
+    """Counter that keys the Gumbel draw of successive STListNet and MDPRank calls (same role as the tie-shuffle counter)."""
     global _noise_offset
     _noise_offset += 1
     return _noise_offset

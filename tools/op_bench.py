@@ -52,6 +52,10 @@ for name, params, shapes in [
     ("WassRank", dict(cost_type="eg"), [(1024, 256), (256, 1024)]),      # default settings: label-group schedule
     ("WassRank", dict(cost_type="ddg"), [(1024, 256)]),                  # O(n^2) walks
     ("WassRank", dict(cost_type="p1"), [(256, 1024)]),
+    ("MDPRank", dict(distribution="PL", top_k=10), [(1024, 256), (256, 1024), (64, 4096)]),
+    ("MDPRank", dict(distribution="PL", top_k=None), [(1024, 256), (256, 1024), (64, 4096)]),
+    ("MDPRank", dict(distribution="STPL", top_k=10), [(1024, 256), (256, 1024), (64, 4096)]),
+    ("MDPRank", dict(distribution="STPL", top_k=None), [(1024, 256), (256, 1024), (64, 4096)]),
 ]:
     for (B, n) in shapes:
         s = torch.sigmoid(torch.randn(B, n, device=dev))
@@ -59,11 +63,14 @@ for name, params, shapes in [
         kw = dict(params)
         if name == "ListMLE":
             kw["perm"] = ops.shuffle_ties_perm(y, seed=1, offset=1)
-        if name == "STListNet":
+        if name in ("STListNet", "MDPRank"):
             kw.update(seed=1, offset=1)
         ms = timeit(lambda: ops.rank_loss_and_grad(name, s, y, **kw))
         algo = (16 if name == "ListMLE" else 12) * n * B
-        rows.append((f"{name} {params.get('loss_type', params.get('cost_type', ''))} {('k=%d' % params['k']) if 'k' in params else ''}".strip(), f"B={B} n={n}",
+        tag = params.get('loss_type', params.get('cost_type', params.get('distribution', '')))
+        if name == "MDPRank":
+            tag += " k=%s" % (params['top_k'] or "n")
+        rows.append((f"{name} {tag} {('k=%d' % params['k']) if 'k' in params else ''}".strip(), f"B={B} n={n}",
                      ms, B / ms * 1e3, algo / ms / 1e6, algo / ms / 1e6 / HBM))
 # ndcg / all metrics
 for (B, n) in [(1024, 256), (256, 1024)]:
@@ -111,6 +118,12 @@ for (B, n) in [(1024, 256), (256, 1024), (4096, 32)]:
         rw.init(); rw.train_mode()
         ms_w = timeit(lambda: rw.train_op(X, y, presort=True, label_type=LABEL_TYPE.MultiLabel, epoch_k=1))
         rows.append(("WassRank train step (fwd+loss+bwd+Adam)", f"B={B} n={n}", ms_w, B / ms_w * 1e3, algo / ms_w / 1e6, algo / ms_w / 1e6 / HBM))
+        # and with MDPRank's default settings (PL, top_k 10, gamma 1, T 1)
+        rm = ptranking_b200.MDPRank(sf_para_dict=sf, model_para_dict=dict(model_id="MDPRank", temperature=1.0, gamma=1.0, top_k=10,
+                                                                          distribution="PL"), gpu=True, device=dev)
+        rm.init(); rm.train_mode()
+        ms_m = timeit(lambda: rm.train_op(X, y, presort=True, label_type=LABEL_TYPE.MultiLabel, epoch_k=1))
+        rows.append(("MDPRank train step (fwd+loss+bwd+Adam)", f"B={B} n={n}", ms_m, B / ms_m * 1e3, algo / ms_m / 1e6, algo / ms_m / 1e6 / HBM))
 # the same step on the ragged batch (batch-level BN: one long list to the scorer, per-query offsets to the loss)
 Xr = torch.randn(total, 136, device=dev)
 ms_s = timeit(lambda: r.train_op(Xr, y_r, presort=True, label_type=LABEL_TYPE.MultiLabel, epoch_k=1, offsets=off_d, max_len=int(lens.max()), buckets=buckets))
