@@ -43,6 +43,7 @@ extern "C" {
 #define PTRB200_MAX_LIST_LEN  4096   /* docs per query handled by the per-list kernels */
 #define PTRB200_MAX_FF_LAYERS   16   /* linear layers in one stacked feed-forward net */
 #define PTRB200_MAX_CUTOFFS     32   /* nDCG cutoffs per call */
+#define PTRB200_MAX_SUBTOPICS   32   /* subtopic rows per query handled by the diversification kernels */
 
 typedef void* ptrb200_stream_t;
 
@@ -197,6 +198,41 @@ int ptrb200_standard_scale(const float* X, const int32_t* offsets, float* out, i
  * even at the store -- scaling first, because raw LETOR features lose precision in bf16.  out must not alias X. */
 int ptrb200_standard_scale_bf16(const float* X, const int32_t* offsets, uint16_t* out, int B, int n, int F,
                                 int clip, float clip_max, ptrb200_stream_t stream);
+
+/* ---- search-result diversification (ptranking/ltr_diversification/) ----------------------------------- */
+/* Subtopic relevance of a ragged batch: query q's q_doc_rele_mat is a dense row-major [sub_counts[q], n_q] fp32 block
+ * that starts at element rele_offsets[q] of `rele` (documents in the query's presorted, ideal order; entries are
+ * non-negative, 0/1 in DIVDataset).  n_q comes from `offsets` (B+1 int32 prefix offsets, or NULL for a dense [B,n]
+ * batch, as for the losses).  n is the longest list and m the largest sub_counts[q] of the batch: host values that size
+ * the launch, so nothing is read back; n <= PTRB200_MAX_LIST_LEN, 1 <= m <= PTRB200_MAX_SUBTOPICS, otherwise
+ * PTRB200_ERR_UNSUPPORTED / PTRB200_ERR_INVALID.  An empty list gives 0. */
+
+/* alphaDCG_as_a_loss, ltr_diversification/score_and_sort/daletor.py:8-40 (+ robust_sigmoid, base/utils.py:57-92):
+ * loss_per_query[q] = -sum over the first min(top_k, m_q) subtopic rows (all rows when top_k <= 0; the reference's
+ * top_k slices rows, not documents) of R_si (1-alpha)^C_si / log2(1 + pi_i), with the sigmoid rank pi and prior cover
+ * counts C of scale rt; grad = d loss_per_query[q] / d scores.  0 <= alpha < 1.  One CTA of fixed width per query, no
+ * atomics: a query's results are bit-identical alone or in any batch. */
+int ptrb200_daletor_fwd_bwd(const float* scores, const int32_t* offsets, const float* rele, const int64_t* rele_offsets,
+                            const int32_t* sub_counts, float* grad, float* loss_per_query, int B, int n, int m, float rt,
+                            float alpha, int top_k, ptrb200_stream_t stream);
+
+/* torch_alpha_ndcg_at_ks / torch_err_ia_at_ks / torch_nerr_ia_at_ks (metric/srd/diversity_metric.py:50-103, 190-290)
+ * after the evaluator's score sort (base/ranker.py:265-475): out[B][3][nks] = alpha-nDCG, ERR-IA, nERR-IA of the
+ * ranking by score (descending, ties by ascending index) against the input order as the ideal; cutoffs > n_q give 0.
+ * ERR-IA's satisfaction is (2^r - 1) / 2^max_label, and it is divided by the query's full m_q.  flags[q] gets
+ * PTRB200_SRD_RELE_GE1 when sum(R) >= 1 and PTRB200_SRD_RELE_GT0 when sum(R) > 0 (the evaluator's skip rules).
+ * order[B,n] (optional) receives the ranking.  ks: host pointer, ascending. */
+#define PTRB200_SRD_RELE_GE1 1
+#define PTRB200_SRD_RELE_GT0 2
+int ptrb200_srd_metrics_at_ks(const float* scores, const int32_t* offsets, const float* rele, const int64_t* rele_offsets,
+                              const int32_t* sub_counts, const int32_t* ks_host, int nks, float* out, int32_t* flags,
+                              int32_t* order, int B, int n, int m, float alpha, float max_label, ptrb200_stream_t stream);
+
+/* DivPointNeuralRanker.div_forward's input, ltr_diversification/base/div_point_ranker.py:14-19: for every document of
+ * query q, out[row] = [q_repr[q], q_repr[q] * docs[row], docs[row]] (width 3F).  docs/out: [B,n,F]/[B,n,3F] dense or
+ * flat rows cut by offsets. */
+int ptrb200_div_features(const float* q_repr, const float* docs, const int32_t* offsets, float* out, int B, int n, int F,
+                         ptrb200_stream_t stream);
 
 /* ---- stacked feed-forward scorer (pointwise MLP; also the head/tail nets of listsf) ---- */
 /* get_stacked_FFNet, ptranking/base/utils.py:288-356; PointNeuralRanker.forward,

@@ -4,6 +4,9 @@
     ptranking_b200.install()           # swap the loss classes into ptranking.ltr_adhoc.eval.ltr
     LTREvaluator(cuda=0).run(model_id='LambdaRank', ...)   # the unmodified reference driver
 
+    ptranking_b200.install_diversification()   # DALETOR into ptranking.ltr_diversification.eval.ltr_diversification
+    DivLTREvaluator(cuda=0).run(model_id='DALETOR', sf_id='pointsf', ...)
+
 Importing the package never touches the GPU; the first kernel call loads
 lib/libptranking_b200.so and raises if it (or an sm_90 device) is missing.
 """
@@ -19,10 +22,12 @@ from .ltr_adhoc.listwise.st_listnet import STListNet
 from .ltr_adhoc.listwise.softrank import SoftRank
 from .ltr_adhoc.listwise.wassrank import WassRank
 from .ltr_adhoc.listwise.mdprank import MDPRank
+from .ltr_diversification.score_and_sort.daletor import DALETOR
 from .base.ranker import LABEL_TYPE
 
 MODELS = {c.__name__: c for c in (RankNet, LambdaRank, LambdaLoss, ListNet, ListMLE, ApproxNDCG,
                                   RankMSE, RankCosine, STListNet, SoftRank, WassRank, MDPRank)}
+DIV_MODELS = {c.__name__: c for c in (DALETOR,)}
 __version__ = "0.1.0"
 
 
@@ -45,4 +50,16 @@ def install(module=None):
         else:
             previous['MDPRankParameter'] = getattr(module, 'MDPRankParameter', None)
             setattr(module, 'MDPRankParameter', MDPRankParameter)
+    return previous
+
+
+def install_diversification(module=None):
+    """Register the diversification classes where the reference's diversification driver resolves model ids by name:
+    ``globals()[model_id]`` in ptranking/ltr_diversification/eval/ltr_diversification.py:385-389."""
+    if module is None:
+        import ptranking.ltr_diversification.eval.ltr_diversification as module  # the reference must be importable
+    previous = {}
+    for name, cls in DIV_MODELS.items():
+        previous[name] = getattr(module, name, None)
+        setattr(module, name, cls)
     return previous

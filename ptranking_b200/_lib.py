@@ -14,6 +14,7 @@ LIB_PATH = os.path.join(_PKG, "lib", "libptranking_b200.so")
 MAX_FF_LAYERS = 16
 MAX_CUTOFFS = 32
 MAX_LIST_LEN = 4096
+MAX_SUBTOPICS = 32
 
 AF_CODES = {None: 0, "R": 1, "GE": 2, "S": 3, "T": 4, "CE": 5, "E": 6, "LR": 7, "SE": 8}
 NORM_CODES = {None: 0, "BN": 1, "BN2": 2}
@@ -75,6 +76,10 @@ SIGNATURES = {
     "ptrb200_sinkstep": (_I, [_fp, _fp, _fp, _fp, _I, _I, _I, _F, _fp]),
     "ptrb200_wassrank_fwd_bwd": (_I, [_fp, _fp, _fp, _fp, _fp, _I, _I, _I, _I, _F, _I, _F, _F, _F, _fp]),
     "ptrb200_mdprank_fwd_bwd": (_I, [_fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _I, _I, _I, _F, _F, _I, _U64, _U64, _fp]),
+    "ptrb200_daletor_fwd_bwd": (_I, [_fp, _fp, _fp, _fp, _fp, _fp, _fp, _I, _I, _I, _F, _F, _I, _fp]),
+    "ptrb200_srd_metrics_at_ks": (_I, [_fp, _fp, _fp, _fp, _fp, C.POINTER(C.c_int32), _I, _fp, _fp, _fp, _I, _I, _I, _F,
+                                       _F, _fp]),
+    "ptrb200_div_features": (_I, [_fp, _fp, _fp, _fp, _I, _I, _I, _fp]),
     "ptrb200_standard_scale": (_I, [_fp, _fp, _fp, _I, _I, _I, _I, _F, _fp]),
     "ptrb200_sum_f32": (_I, [_fp, _fp, _I, _fp]),
     "ptrb200_ndcg_at_ks": (_I, [_fp, _fp, _fp, C.POINTER(C.c_int32), _I, _fp, _fp, _I, _I, _I, _fp]),

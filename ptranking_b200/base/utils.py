@@ -44,7 +44,11 @@ class StackedFFNet(nn.Module):
     """Dropout -> Linear -> (BN|BN2) -> AF per hidden layer, Linear [-> norm -> TL_AF] tail."""
 
     def __init__(self, ff_dims, AF=None, TL_AF=None, apply_tl_af=False, dropout=0.1,
-                 BN=True, bn_type=None, bn_affine=False, device=None, math_mode=None):
+                 BN=True, bn_type=None, bn_affine=False, device=None, math_mode=None, bn_per_query=False):
+        """``bn_per_query`` (bn_type 'BN' only): normalise each query over its own documents, as the reference's BN does
+        when it scores one query per call (the diversification rankers).  The parameters and checkpoint keys stay
+        LTRBatchNorm's; the kernels run BN2's per-query statistics with gamma/beta = bn.weight/bn.bias (constant 1 / 0
+        without affine) and no second affine."""
         super().__init__()
         # "3xtf32" (default): wgmma tensor cores with the fp32-equivalent 3-pass TF32 split;
         # "tf32": single pass; "simt": fp32 FMA kernels (also the fallback for widths the MMA tiles reject)
@@ -55,8 +59,13 @@ class StackedFFNet(nn.Module):
                 raise NotImplementedError(f"activation {code!r}")     # get_AF's broken / unsupported branches
         if BN and bn_type not in ("BN", "BN2"):
             raise NotImplementedError(bn_type)
+        if bn_per_query and not (BN and bn_type == "BN"):
+            raise ValueError("bn_per_query applies to bn_type='BN' only")
         L = len(ff_dims)
-        self._order = []            # parameter tensors in the order the C ABI expects them
+        self._const_grads = []      # gradient sinks of the constant gamma/beta of a non-affine per-query BN
+        # parameter tensors in the order the C ABI expects them; (module, buffer) names stand for those constants, which
+        # .to() replaces
+        self._order = []
         for i in range(1, L):
             lin = nn.Linear(ff_dims[i - 1], ff_dims[i])
             nn.init.xavier_normal_(lin.weight)
@@ -68,17 +77,41 @@ class StackedFFNet(nn.Module):
                     holder = _BNParams(ff_dims[i], bn_affine)
                     if bn_affine:
                         self._order += [holder.bn.weight, holder.bn.bias]
+                    elif bn_per_query:
+                        holder.register_buffer("unit_gamma", torch.ones(ff_dims[i]), persistent=False)
+                        holder.register_buffer("zero_beta", torch.zeros(ff_dims[i]), persistent=False)
+                        self._order += [(f"bn_{i + 1}", "unit_gamma"), (f"bn_{i + 1}", "zero_beta")]
                 else:
                     holder = _BN2Params(ff_dims[i], bn_affine, device=device)
                     self._order += [holder.gamma, holder.beta]
                     if bn_affine:
                         self._order += [holder.weight, holder.bias]
                 self.add_module(f"bn_{i + 1}", holder)
+        self.bn_per_query = bool(bn_per_query)
+        norm = ("BN2" if bn_per_query else bn_type) if BN else None
         self.spec = ops.FFNetSpec(ff_dims, AF if L > 2 else None, TL_AF if apply_tl_af else None,
-                                  bn_type if BN else None, bn_affine, dropout, math_mode=math_mode)
+                                  norm, bn_affine and not bn_per_query, dropout, math_mode=math_mode)
 
     def ordered_parameters(self):
-        return list(self._order)
+        return [getattr(getattr(self, e[0]), e[1]) if isinstance(e, tuple) else e for e in self._order]
+
+    def _grad_targets(self):
+        """p.grad of every parameter, and a scratch sink for each constant -- or None while some gradient storage is
+        missing."""
+        targets = []
+        consts = 0
+        for p in self.ordered_parameters():
+            if isinstance(p, nn.Parameter):
+                if p.grad is None or not p.grad.is_contiguous():
+                    return None
+                targets.append(p.grad)
+            else:
+                if consts == len(self._const_grads) or self._const_grads[consts].shape != p.shape \
+                        or self._const_grads[consts].device != p.device:
+                    self._const_grads[consts:consts + 1] = [torch.empty_like(p)]
+                targets.append(self._const_grads[consts])
+                consts += 1
+        return targets
 
     def forward(self, X, offsets=None, max_len=None):
         """[B,n,F] (or [rows,F]) -> [B,n,out].  ``offsets``/``max_len`` describe a ragged batch ([total_docs,F] rows cut
@@ -90,15 +123,14 @@ class StackedFFNet(nn.Module):
         # when every parameter already owns gradient storage (the ranker's flat bucket), the backward kernels write
         # into it directly instead of handing autograd 2 tensors per layer to accumulate
         targets = None
-        if torch.is_grad_enabled() and all(p.grad is not None and p.grad.is_contiguous() for p in self._order) \
-                and getattr(self, "write_through_grads", False):
-            targets = [p.grad for p in self._order]
+        if torch.is_grad_enabled() and getattr(self, "write_through_grads", False):
+            targets = self._grad_targets()
         if ragged_bn2:
             if X.dim() != 2:
                 raise ValueError("a ragged batch is [total_docs, F]")
-            return ops.ffnet_apply(X, self.spec, self._order, training=self.training, grad_targets=targets,
+            return ops.ffnet_apply(X, self.spec, self.ordered_parameters(), training=self.training, grad_targets=targets,
                                    offsets=offsets, max_len=max_len)
-        out = ops.ffnet_apply(X, self.spec, self._order, training=self.training, grad_targets=targets)
+        out = ops.ffnet_apply(X, self.spec, self.ordered_parameters(), training=self.training, grad_targets=targets)
         return out.squeeze(0) if squeeze else out
 
 

@@ -494,14 +494,6 @@ __global__ void shuffle_ties_kernel(const float* __restrict__ labels, int32_t* _
 // ---------------------------------------------------------------------------
 // ApproxNDCG
 // ---------------------------------------------------------------------------
-// Robust_Sigmoid forward, base/utils.py:62-78 (branch on the sign of the unscaled input)
-static __device__ __forceinline__ float robust_sigmoid(float in, float alpha) {
-    const float x = alpha * in;
-    if (in > 0.0f) return __fdividef(1.0f, 1.0f + expf(-x));
-    if (in < 0.0f) { const float ex = expf(x); return __fdividef(ex, 1.0f + ex); }
-    return 0.5f;
-}
-
 __global__ void inv_idcg_kernel(const float* __restrict__ labels, float* __restrict__ inv_idcg, const int32_t* __restrict__ offsets,
                                 int nmax, int npow2max, int presort) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -564,8 +556,6 @@ __global__ void sum_kernel(const float* __restrict__ x, float* __restrict__ out,
     v = block_sum(v, red);
     if (threadIdx.x == 0) out[0] = v;
 }
-
-struct Cutoffs { int k[PTRB200_MAX_CUTOFFS]; int n; };
 
 __global__ void ndcg_at_ks_kernel(const float* __restrict__ scores, const float* __restrict__ labels,
                                   Cutoffs ks, float* __restrict__ out, int32_t* __restrict__ order, const int32_t* __restrict__ offsets,

@@ -1,5 +1,5 @@
-// losses_common.cuh -- helpers shared by the per-list kernels (losses.cu, losses_ext.cu): list addressing for uniform
-// and ragged batches, iDCG, block scans, host-side launch checks.
+// losses_common.cuh -- helpers shared by the per-list kernels (losses.cu, losses_ext.cu, wassrank.cu, diversity.cu): list
+// addressing for uniform and ragged batches, iDCG, the robust sigmoid, metric cutoffs, block scans, host-side launch checks.
 #pragma once
 #include "common.cuh"
 
@@ -35,6 +35,17 @@ static __device__ float block_idcg(const float* __restrict__ y, int n, int npow2
     }
     return block_sum(part, red);
 }
+
+// Robust_Sigmoid forward, base/utils.py:62-78 (branch on the sign of the unscaled input)
+static __device__ __forceinline__ float robust_sigmoid(float in, float alpha) {
+    const float x = alpha * in;
+    if (in > 0.0f) return __fdividef(1.0f, 1.0f + expf(-x));
+    if (in < 0.0f) { const float ex = expf(x); return __fdividef(ex, 1.0f + ex); }
+    return 0.5f;
+}
+
+// metric cutoffs, ascending, passed by value to the metric kernels
+struct Cutoffs { int k[PTRB200_MAX_CUTOFFS]; int n; };
 
 // ---------------------------------------------------------------------------
 // block-wide inclusive scan over a shared-memory array (forward or reverse)

@@ -504,6 +504,147 @@ def adhoc_metrics_at_ks(scores: torch.Tensor, labels: torch.Tensor, ks: Sequence
 
 
 # --------------------------------------------------------------------------- #
+# search-result diversification: subtopic relevance blocks, DALETOR loss, alpha-nDCG / (n)ERR-IA, scorer input
+# --------------------------------------------------------------------------- #
+class SubtopicRele:
+    """Subtopic relevance of a batch in the layout the diversification kernels read: query q's q_doc_rele_mat
+    ([m_q, n_q], documents in presorted order) as a row-major block of the flat fp32 ``rele`` starting at element
+    ``rele_offsets[q]`` (int64), ``sub_counts[q]`` = m_q (int32), all on the device; ``max_sub`` = max m_q (host int)."""
+
+    def __init__(self, rele, rele_offsets, sub_counts, max_sub):
+        self.rele, self.rele_offsets, self.sub_counts, self.max_sub = rele, rele_offsets, sub_counts, int(max_sub)
+
+    @classmethod
+    def pack(cls, mats: Sequence[torch.Tensor], device) -> "SubtopicRele":
+        """One host->device copy of the [m_q, n_q] matrices of a batch."""
+        sizes = [int(r.numel()) for r in mats]
+        offs = [0]
+        for sz in sizes[:-1]:
+            offs.append(offs[-1] + sz)
+        flat = torch.cat([r.reshape(-1).float().cpu() for r in mats] + [torch.zeros(1)])   # never a null pointer
+        counts = torch.tensor([int(r.shape[0]) for r in mats], dtype=torch.int32)
+        return cls(flat.to(device), torch.tensor(offs, dtype=torch.int64).to(device), counts.to(device),
+                   max((int(r.shape[0]) for r in mats), default=0))
+
+    def select(self, q0: int, q1: int) -> "SubtopicRele":
+        """Queries [q0, q1) of the batch (the blocks stay where they are)."""
+        return SubtopicRele(self.rele, self.rele_offsets[q0:q1], self.sub_counts[q0:q1], self.max_sub)
+
+    def _ptrs(self, device):
+        for t, name in ((self.rele, "rele"), (self.rele_offsets, "rele_offsets"), (self.sub_counts, "sub_counts")):
+            if not t.is_cuda or t.device != device:
+                raise _lib.B200LibraryError(f"{name} must live on the device of the scores")
+        if self.rele.dtype != torch.float32 or self.rele_offsets.dtype != torch.int64 or self.sub_counts.dtype != torch.int32:
+            raise ValueError("rele / rele_offsets / sub_counts must be float32 / int64 / int32")
+        if not (self.rele.is_contiguous() and self.rele_offsets.is_contiguous() and self.sub_counts.is_contiguous()):
+            raise ValueError("rele / rele_offsets / sub_counts must be contiguous")
+        return self.rele.data_ptr(), self.rele_offsets.data_ptr(), self.sub_counts.data_ptr()
+
+
+@_on_tensor_device
+def daletor_loss_and_grad(scores: torch.Tensor, rele: SubtopicRele, rt: float = 10.0, top_k: Optional[int] = 10,
+                          alpha: float = 0.5, offsets: Optional[torch.Tensor] = None, max_len: Optional[int] = None):
+    """DALETOR's alphaDCG_as_a_loss (daletor.py:22-40) for every query of a batch in one launch -> (batch loss = sum of
+    the per-query losses, per-query losses [B], d loss / d scores).  ``top_k`` slices subtopic rows, as the reference
+    does; ``None`` (or <= 0) takes them all.  Scores: [B,n] dense or flat with ``offsets``/``max_len``."""
+    lib = _lib.load()
+    s = _dev_f32(scores, "scores")
+    B, n, offsets, op = _list_layout(s, offsets, max_len)
+    if rele.sub_counts.numel() != B:
+        raise ValueError(f"{rele.sub_counts.numel()} subtopic blocks for {B} queries")
+    rp, rop, scp = rele._ptrs(s.device)
+    grad = torch.empty_like(s)
+    loss_q = torch.empty(B, dtype=torch.float32, device=s.device)
+    _lib.check(lib.ptrb200_daletor_fwd_bwd(s.data_ptr(), op, rp, rop, scp, grad.data_ptr(), loss_q.data_ptr(), B, n,
+                                           max(rele.max_sub, 1), float(rt), float(alpha), int(top_k) if top_k else 0,
+                                           _stream_ptr()), "daletor loss kernel")
+    return sum_f32(loss_q), loss_q, grad
+
+
+class _DaletorLoss(torch.autograd.Function):
+    """batch loss = sum of per-query DALETOR losses; backward hands the fused gradient to the scorer (as _RankLoss)."""
+
+    @staticmethod
+    @_on_tensor_device
+    def forward(ctx, scores, rele, params):
+        loss, loss_q, grad = daletor_loss_and_grad(scores.detach(), rele, **params)
+        ctx.save_for_backward(grad)
+        ctx.mark_non_differentiable(loss_q)
+        ctx.set_materialize_grads(False)
+        return loss, loss_q
+
+    @staticmethod
+    @_on_tensor_device
+    def backward(ctx, g_loss, _g_lq):
+        (grad,) = ctx.saved_tensors
+        if g_loss is None:
+            return None, None, None
+        return _ew(EW_MUL_SCALAR, grad, g_loss.reshape(1)), None, None
+
+
+def daletor_loss(scores: torch.Tensor, rele: SubtopicRele, **params):
+    """(0-dim batch loss differentiable w.r.t. ``scores``, per-query losses [B]); ``params`` as daletor_loss_and_grad."""
+    return _DaletorLoss.apply(scores, rele, params)
+
+
+@_on_tensor_device
+def srd_metrics_at_ks(scores: torch.Tensor, rele: SubtopicRele, ks: Sequence[int], max_label: float, alpha: float = 0.5,
+                      offsets: Optional[torch.Tensor] = None, max_len: Optional[int] = None, return_order: bool = False):
+    """alpha-nDCG, ERR-IA and nERR-IA at the cutoffs ``ks`` of the ranking by score (ideal order: the input order) for
+    every query from one kernel -> (andcg, err_ia, nerr_ia: [B, len(ks)], flags [B] int32[, order]).  Cutoffs beyond a
+    list's length give 0.  ``flags`` bit 0: sum(R) >= 1, bit 1: sum(R) > 0 (the evaluator's skip rules)."""
+    assert max_label is not None   # torch_rankwise_err_ia's assert (diversity_metric.py:193)
+    lib = _lib.load()
+    s = _dev_f32(scores, "scores")
+    B, n, offsets, op = _list_layout(s, offsets, max_len)
+    if rele.sub_counts.numel() != B:
+        raise ValueError(f"{rele.sub_counts.numel()} subtopic blocks for {B} queries")
+    rp, rop, scp = rele._ptrs(s.device)
+    ks = [int(k) for k in ks]
+    order_ix = sorted(range(len(ks)), key=lambda i: ks[i])
+    arr = (C.c_int32 * len(ks))(*[ks[i] for i in order_ix])
+    out = torch.empty((B, 3, len(ks)), dtype=torch.float32, device=s.device)
+    flags = torch.empty(B, dtype=torch.int32, device=s.device)
+    order = torch.empty(s.shape, dtype=torch.int32, device=s.device) if return_order else None
+    _lib.check(lib.ptrb200_srd_metrics_at_ks(s.data_ptr(), op, rp, rop, scp, arr, len(ks), out.data_ptr(), flags.data_ptr(),
+                                             order.data_ptr() if return_order else None, B, n, max(rele.max_sub, 1),
+                                             float(alpha), float(max_label), _stream_ptr()), "srd_metrics_at_ks")
+    if order_ix != list(range(len(ks))):
+        inv = torch.empty(len(ks), dtype=torch.long)
+        inv[torch.tensor(order_ix)] = torch.arange(len(ks))
+        out = out[:, :, inv.to(out.device)]
+    res = (out[:, 0], out[:, 1], out[:, 2], flags)
+    return (*res, order) if return_order else res
+
+
+@_on_tensor_device
+def div_features(q_repr: torch.Tensor, docs: torch.Tensor, offsets: Optional[torch.Tensor] = None,
+                 max_len: Optional[int] = None) -> torch.Tensor:
+    """[q, q*d, d] rows of the pointwise diversification scorer (div_point_ranker.py:14-19).  q_repr: [B,F]; docs:
+    [B,n,F] dense or flat [total_docs,F] with ``offsets``/``max_len`` -> the same layout with width 3F.  Forward only:
+    both inputs are data."""
+    lib = _lib.load()
+    q, d = _dev_f32(q_repr, "q_repr"), _dev_f32(docs, "docs")
+    F = d.shape[-1]
+    if offsets is None:
+        if d.dim() != 3:
+            raise ValueError(f"expected [B,n,F] documents, got {tuple(d.shape)}")
+        B, n, op = d.shape[0], d.shape[1], None
+    else:
+        if d.dim() != 2 or max_len is None:
+            raise ValueError("ragged documents are [total_docs, F] with offsets= and max_len=")
+        offsets = offsets.to(device=d.device, dtype=torch.int32).contiguous()
+        B, n, op = offsets.numel() - 1, max(int(max_len), 1), offsets.data_ptr()
+    if q.shape != (B, F):
+        raise ValueError(f"q_repr {tuple(q.shape)} does not match {B} queries of width {F}")
+    out = torch.empty((*d.shape[:-1], 3 * F), dtype=torch.float32, device=d.device)
+    if d.numel():
+        _lib.check(lib.ptrb200_div_features(q.data_ptr(), d.data_ptr(), op, out.data_ptr(), B, n, F, _stream_ptr()),
+                   "div_features")
+    return out
+
+
+# --------------------------------------------------------------------------- #
 # stacked feed-forward scorer
 # --------------------------------------------------------------------------- #
 _dropout_offset = 0

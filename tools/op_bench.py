@@ -72,6 +72,15 @@ for name, params, shapes in [
             tag += " k=%s" % (params['top_k'] or "n")
         rows.append((f"{name} {tag} {('k=%d' % params['k']) if 'k' in params else ''}".strip(), f"B={B} n={n}",
                      ms, B / ms * 1e3, algo / ms / 1e6, algo / ms / 1e6 / HBM))
+# DALETOR (diversification): m = 8 subtopic rows of 0/1 relevance per query, rt 10, top_k 10 (the reference's defaults)
+for (B, n) in [(1024, 256), (64, 4096)]:
+    s = torch.randn(B, n, device=dev)
+    rele = ops.SubtopicRele.pack([torch.from_numpy((rng.random((8, n)) < 0.2).astype(np.float32)) for _ in range(B)], dev)
+    ms = timeit(lambda: ops.daletor_loss_and_grad(s, rele, rt=10.0, top_k=10))
+    algo = (12 + 8 * 4) * n * B
+    rows.append(("DALETOR m=8 k=10", f"B={B} n={n}", ms, B / ms * 1e3, algo / ms / 1e6, algo / ms / 1e6 / HBM))
+    ms = timeit(lambda: ops.srd_metrics_at_ks(s, rele, [1, 3, 5, 10, 20], max_label=1.0))
+    rows.append(("alpha-nDCG+ERR-IA+nERR-IA @5 cutoffs m=8", f"B={B} n={n}", ms, B / ms * 1e3, algo / ms / 1e6, algo / ms / 1e6 / HBM))
 # ndcg / all metrics
 for (B, n) in [(1024, 256), (256, 1024)]:
     s = torch.randn(B, n, device=dev); y = labels(B, n)
@@ -124,6 +133,24 @@ for (B, n) in [(1024, 256), (256, 1024), (4096, 32)]:
         rm.init(); rm.train_mode()
         ms_m = timeit(lambda: rm.train_op(X, y, presort=True, label_type=LABEL_TYPE.MultiLabel, epoch_k=1))
         rows.append(("MDPRank train step (fwd+loss+bwd+Adam)", f"B={B} n={n}", ms_m, B / ms_m * 1e3, algo / ms_m / 1e6, algo / ms_m / 1e6 / HBM))
+# DALETOR with the default diversification pointsf (F = 100, so 300 inputs; 5 x 100 GELU, per-query BN; Adagrad): the
+# reference's one query per step, and 1024 queries in one ragged step (queries_per_step = 1024)
+sfd = dict(sf_id="pointsf", opt="Adagrad", lr=0.001, pointsf=dict(num_features=100, num_layers=5, AF="GE", TL_AF="GE",
+                                                                  apply_tl_af=False, BN=True, bn_type="BN", bn_affine=True))
+rd = ptranking_b200.DALETOR(sf_para_dict=sfd, model_para_dict=dict(model_id="DALETOR", rt=10.0, top_k=10), gpu=True, device=dev)
+rd.init(); rd.train_mode()
+for (B, n) in [(1, 256), (1024, 256)]:
+    Xd = torch.randn(B * n, 300, device=dev)
+    rele = ops.SubtopicRele.pack([torch.from_numpy((rng.random((8, n)) < 0.2).astype(np.float32)) for _ in range(B)], dev)
+    offd = torch.arange(0, (B + 1) * n, n, dtype=torch.int32, device=dev)
+    if B == 1:
+        step = lambda: rd.div_custom_loss_function(rd.point_sf(Xd.view(1, n, 300)).view(1, -1), rele, presort=True)
+    else:
+        step = lambda: rd.div_custom_loss_function(rd.div_forward_ragged(Xd, offd, n), rele, presort=True, offsets=offd, max_len=n)
+    ms_d = timeit(step)
+    algo = B * n * (300 * 4 + 8)
+    rows.append(("DALETOR train step (pointsf 300->5x100, per-query BN, Adagrad)", f"B={B} n={n}", ms_d, B / ms_d * 1e3,
+                 algo / ms_d / 1e6, algo / ms_d / 1e6 / HBM))
 # the same step on the ragged batch (batch-level BN: one long list to the scorer, per-query offsets to the loss)
 Xr = torch.randn(total, 136, device=dev)
 ms_s = timeit(lambda: r.train_op(Xr, y_r, presort=True, label_type=LABEL_TYPE.MultiLabel, epoch_k=1, offsets=off_d, max_len=int(lens.max()), buckets=buckets))
