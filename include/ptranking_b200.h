@@ -234,6 +234,24 @@ int ptrb200_srd_metrics_at_ks(const float* scores, const int32_t* offsets, const
 int ptrb200_div_features(const float* q_repr, const float* docs, const int32_t* offsets, float* out, int B, int n, int F,
                          ptrb200_stream_t stream);
 
+/* DivListNeuralRanker.div_forward's encoder input, ltr_diversification/base/div_list_ranker.py:61-64: out[row] =
+ * [q_repr[q], docs[row], q_repr[q] * docs[row]] (width 3F; d before q*d, unlike ptrb200_div_features).  Layouts as
+ * ptrb200_div_features. */
+int ptrb200_div_list_features(const float* q_repr, const float* docs, const int32_t* offsets, float* out, int B, int n,
+                              int F, ptrb200_stream_t stream);
+
+/* One length class of a ragged batch (flat rows cut by the B_all+1 int32 prefix offsets): class query b is query qidx[b]
+ * (qidx: B int32 on the device, or NULL for queries 0..B-1), every list of the class has at most n_max rows.
+ * ptrb200_pad_lists_pitched: padded[b, r, 0:W] = src[(offsets[q] + r) * ld_src + 0:W] for the list's rows, 0 behind
+ * them -- a strided column block of the rows (ld_src >= W) into the dense [B, n_max, W] layout of the encoder.
+ * ptrb200_div_list_concat: the uni_sf input of the class's rows, div_list_ranker.py:80: out[row, 0:W] = feats[row, 0:W]
+ * and out[row, W:2W] = enc[b, r, 0:W] (enc: the encoder's padded [B, n_max, W] output; out rows are 2W wide).  Its
+ * backward is ptrb200_pad_lists_pitched on columns W:2W of the gradient (src = grad + W, ld_src = 2W). */
+int ptrb200_pad_lists_pitched(const float* src, long long ld_src, const int32_t* offsets, const int32_t* qidx,
+                              float* padded, int B, int n_max, int W, ptrb200_stream_t stream);
+int ptrb200_div_list_concat(const float* feats, const float* enc, const int32_t* offsets, const int32_t* qidx, float* out,
+                            int B, int n_max, int W, ptrb200_stream_t stream);
+
 /* ---- stacked feed-forward scorer (pointwise MLP; also the head/tail nets of listsf) ---- */
 /* get_stacked_FFNet, ptranking/base/utils.py:288-356; PointNeuralRanker.forward,
  * base/point_ranker.py:45-55; LTRBatchNorm / LTRBatchNorm2, base/utils.py:201-282;

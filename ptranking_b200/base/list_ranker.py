@@ -133,6 +133,18 @@ class Encoder(nn.Module):
         return self.norm(x) if 'AllRank' == self.encoder_type else x
 
 
+def encoder_parameters(encoder):
+    """The encoder's parameters with each attention block's projection weights side by side
+    (MultiheadAttention.projection_parameters), so that a flat parameter buffer holds them as one [3*hid, hid] matrix."""
+    enc, seen = [], set()
+    for m in encoder.modules():
+        if isinstance(m, MultiheadAttention):
+            for p in m.projection_parameters():
+                if id(p) not in seen:
+                    seen.add(id(p)); enc.append(p)
+    return enc + [p for p in encoder.parameters() if id(p) not in seen]
+
+
 class ListNeuralRanker(NeuralRanker):
     """Permutation-equivariant ranker: head FFN, MHSA encoder, tail FFN (list_ranker.py:280-402)."""
 
@@ -149,16 +161,10 @@ class ListNeuralRanker(NeuralRanker):
 
     def get_parameters(self):
         """Same set as the reference (list_ranker.py:297-301); inside the encoder each attention block's projection
-        weights are listed side by side (MultiheadAttention.projection_parameters) -- the order only decides the layout
-        of the flat parameter / gradient buffers, checkpoints are per-module state_dicts."""
-        enc, seen = [], set()
-        for m in self.list_sf['encoder'].modules():
-            if isinstance(m, MultiheadAttention):
-                for p in m.projection_parameters():
-                    if id(p) not in seen:
-                        seen.add(id(p)); enc.append(p)
-        enc += [p for p in self.list_sf['encoder'].parameters() if id(p) not in seen]
-        return list(self.list_sf['head_ffnns'].parameters()) + enc + list(self.list_sf['tail_ffnns'].parameters())
+        weights are listed side by side (encoder_parameters) -- the order only decides the layout of the flat parameter /
+        gradient buffers, checkpoints are per-module state_dicts."""
+        return list(self.list_sf['head_ffnns'].parameters()) + encoder_parameters(self.list_sf['encoder']) + \
+            list(self.list_sf['tail_ffnns'].parameters())
 
     def ini_listsf(self, num_features=None, ff_dims=[128, 256, 512], out_dim=1, AF='R', TL_AF='GE', apply_tl_af=False,
                    BN=True, bn_type=None, bn_affine=False, n_heads=2, encoder_layers=3, dropout=0.1, encoder_type=None):

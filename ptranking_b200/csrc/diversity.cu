@@ -206,6 +206,53 @@ __global__ void div_features_kernel(const float* __restrict__ q_repr, const floa
     }
 }
 
+// ---------------------------------------------------------------------------
+// The diversification list scorer, ltr_diversification/base/div_list_ranker.py:61-85
+// ---------------------------------------------------------------------------
+// Encoder input [q, d, q*d] (note: d before q*d, unlike the pointwise [q, q*d, d]).
+__global__ void div_list_features_kernel(const float* __restrict__ q_repr, const float* __restrict__ docs,
+                                         const int32_t* __restrict__ offsets, float* __restrict__ out, int nmax, int F) {
+    const int b = blockIdx.x;
+    const ListSpan sp = list_span(offsets, b, nmax);
+    const float* q = q_repr + (size_t)b * F;
+    for (size_t e = threadIdx.x; e < (size_t)sp.n * F; e += blockDim.x) {
+        const size_t row = sp.base + e / F;
+        const int f = (int)(e % F);
+        const float qv = q[f], dv = docs[row * F + f];
+        float* orow = out + row * 3 * F;
+        orow[f] = qv;
+        orow[F + f] = dv;
+        orow[2 * F + f] = qv * dv;
+    }
+}
+
+// A length class of a ragged batch: query b of the class is query qidx[b] (b when qidx is NULL) of the prefix offsets,
+// padded to n_max rows.  One CTA per (class query, row block), as pad_lists_kernel.
+//   PAD:  padded[b, r, 0:W] = src[(offsets[q] + r) * ld_src + 0:W] for r < len_q, 0 for len_q <= r < n_max
+//   !PAD: the scorer input of the class's rows: out[row, 0:W] = feats[row, 0:W], out[row, W:2W] = enc[b, r, 0:W]
+template <bool PAD>
+__global__ void div_list_rows_kernel(const float* __restrict__ src, long long ld_src, const float* __restrict__ enc,
+                                     const int32_t* __restrict__ offsets, const int32_t* __restrict__ qidx,
+                                     float* __restrict__ dst, int n_max, int W) {
+    const int b = blockIdx.x;
+    const int q = qidx ? qidx[b] : b;
+    const int base = offsets[q], n = min(offsets[q + 1] - base, n_max);
+    for (int r = blockIdx.y; r < (PAD ? n_max : n); r += gridDim.y) {
+        if (PAD) {
+            const float* s = src + (size_t)(base + r) * ld_src;
+            float* d = dst + ((size_t)b * n_max + r) * W;
+            const bool live = r < n;
+            for (int f = threadIdx.x; f < W; f += blockDim.x) d[f] = live ? s[f] : 0.0f;
+        } else {
+            const size_t row = (size_t)(base + r);
+            const float* s = src + row * W;
+            const float* e = enc + ((size_t)b * n_max + r) * W;
+            float* d = dst + row * 2 * W;
+            for (int f = threadIdx.x; f < W; f += blockDim.x) { d[f] = s[f]; d[W + f] = e[f]; }
+        }
+    }
+}
+
 static int check_rele_args(const char* who, const void* rele, const void* rele_offsets, const void* sub_counts, int m) {
     if (!rele || !rele_offsets || !sub_counts || m <= 0) {
         set_error("%s: null subtopic relevance arguments or non-positive m=%d", who, m);
@@ -273,6 +320,40 @@ int ptrb200_div_features(const float* q_repr, const float* docs, const int32_t* 
     }
     PTRB200_LAUNCH(div_features_kernel, B, 256, 0, stream, q_repr, docs, offsets, out, n, F);
     return check_launch("div_features");
+}
+
+int ptrb200_div_list_features(const float* q_repr, const float* docs, const int32_t* offsets, float* out, int B, int n,
+                              int F, ptrb200_stream_t stream) {
+    if (!q_repr || !docs || !out || B <= 0 || n <= 0 || F <= 0) {
+        set_error("div_list_features: null pointer or non-positive size (B=%d n=%d F=%d)", B, n, F);
+        return PTRB200_ERR_INVALID;
+    }
+    PTRB200_LAUNCH(div_list_features_kernel, B, 256, 0, stream, q_repr, docs, offsets, out, n, F);
+    return check_launch("div_list_features");
+}
+
+static inline int div_list_threads(int W) { return W >= 128 ? 128 : ((W + 31) / 32) * 32; }
+
+int ptrb200_pad_lists_pitched(const float* src, long long ld_src, const int32_t* offsets, const int32_t* qidx,
+                              float* padded, int B, int n_max, int W, ptrb200_stream_t stream) {
+    if (!src || !offsets || !padded || B <= 0 || n_max <= 0 || W <= 0 || ld_src < W) {
+        set_error("pad_lists_pitched: bad arguments (B=%d n_max=%d W=%d ld_src=%lld)", B, n_max, W, ld_src);
+        return PTRB200_ERR_INVALID;
+    }
+    PTRB200_LAUNCH_TAG("pad_lists_pitched_kernel", div_list_rows_kernel<true>, dim3(B, n_max < 64 ? n_max : 64), div_list_threads(W), 0, stream, src,
+                   ld_src, nullptr, offsets, qidx, padded, n_max, W);
+    return check_launch("pad_lists_pitched");
+}
+
+int ptrb200_div_list_concat(const float* feats, const float* enc, const int32_t* offsets, const int32_t* qidx, float* out,
+                            int B, int n_max, int W, ptrb200_stream_t stream) {
+    if (!feats || !enc || !offsets || !out || B <= 0 || n_max <= 0 || W <= 0) {
+        set_error("div_list_concat: bad arguments (B=%d n_max=%d W=%d)", B, n_max, W);
+        return PTRB200_ERR_INVALID;
+    }
+    PTRB200_LAUNCH_TAG("div_list_concat_kernel", div_list_rows_kernel<false>, dim3(B, n_max < 64 ? n_max : 64), div_list_threads(W), 0, stream, feats,
+                   (long long)W, enc, offsets, qidx, out, n_max, W);
+    return check_launch("div_list_concat");
 }
 
 }  // extern "C"

@@ -1,15 +1,19 @@
-"""DiversityNeuralRanker with the pointwise scorer (mirror of ptranking/ltr_diversification/base/diversity_ranker.py,
-div_point_ranker.py and the diversified-ranking methods of base/ranker.py:265-475, :655-700).
+"""DiversityNeuralRanker with the pointwise or the list scorer (mirror of
+ptranking/ltr_diversification/base/diversity_ranker.py, div_point_ranker.py, div_list_ranker.py and the
+diversified-ranking methods of base/ranker.py:265-475, :655-700).
 
 The reference walks a DIVDataset query by query: one scorer forward per query, and for evaluation a device-to-host copy
 and a CPU metric per query.  Here a split is packed once into device tensors -- the [q, q*d, d] scorer input of every
 document (ops.div_features), ragged offsets and the subtopic relevance blocks -- and cached per dataset object.
 Evaluation is one scorer forward and one metric launch per split; training keeps the reference's one step per query by
 default.  The reference's BN normalises each query over its own documents because it scores one query per call; the
-scorer's per-query BN mode (StackedFFNet ``bn_per_query``) keeps that when many queries share a launch.
+scorer's per-query BN mode (StackedFFNet ``bn_per_query``) keeps that when many queries share a launch.  The list
+scorer (sf_id='listsf', div_list_ranker.py) reads the list-order rows [q, d, q*d] instead, which are then the only
+features a listsf ranker builds for a split.
 """
 from __future__ import annotations
 
+import os
 import weakref
 
 import numpy as np
@@ -18,13 +22,15 @@ import torch
 from ... import ops
 from ...base.point_ranker import PointNeuralRanker
 from ...base.utils import StackedFFNet
+from .div_list_ranker import ATTN_BUDGET_BYTES, DivListNeuralRanker, check_listsf_config
 
 
 class _Split:
-    """One DIVDataset on the device: X [total, 3F] scorer input, int32 offsets [Q+1] (device) and their host copy,
-    the subtopic relevance blocks, host qids / perm_docs and the per-query relevance mass (host, for the skip rules)."""
+    """One DIVDataset on the device: X [total, 3F] scorer input ([q, q*d, d]; [q, d, q*d] with ``list_order``, the
+    list scorer's encoder input), int32 offsets [Q+1] (device) and their host copy, the subtopic relevance blocks, host
+    qids / perm_docs and the per-query relevance mass (host, for the skip rules)."""
 
-    def __init__(self, data, device):
+    def __init__(self, data, device, list_order=False):
         qids, perm_docs, q_reprs, docs, mats = [], [], [], [], []
         for qid, q_repr, q_perm_docs, doc_reprs, _alpha_dcg, _subtopics, q_doc_rele_mat in data:
             qids.append(qid)
@@ -43,8 +49,9 @@ class _Split:
         self.rele = ops.SubtopicRele.pack(mats, device)
         q = torch.cat(q_reprs).to(device) if q_reprs else torch.zeros(0, 1, device=device)
         d = torch.cat(docs).to(device) if docs else torch.zeros(0, 1, device=device)
-        self.X = ops.div_features(q, d, offsets=self.offsets, max_len=self.max_len)
-        self._steps = {}
+        build = ops.div_list_features if list_order else ops.div_features
+        self.X = build(q, d, offsets=self.offsets, max_len=self.max_len)
+        self._steps, self._plans = {}, {}
 
     def __len__(self):
         return len(self.qids)
@@ -75,21 +82,44 @@ class _Split:
             self._steps[queries_per_step] = steps
         return self._steps[queries_per_step]
 
+    def plan(self, q0, q1, ranker):
+        """The list scorer's layout of queries [q0, q1) (div_list_ranker.ListPlan), built once per budget."""
+        key = (q0, q1, ranker.attn_budget_bytes)
+        if key not in self._plans:
+            self._plans[key] = ranker.list_plan(self.offsets_host[q0:q1 + 1])
+        return self._plans[key]
 
-class DiversityNeuralRanker(PointNeuralRanker):
-    """pointsf only: the diversification list scorer (AttnDIN, div_list_ranker.py) is not built here yet."""
+
+class DiversityNeuralRanker(PointNeuralRanker, DivListNeuralRanker):
+    """sf_id 'pointsf' (stacked FF net over [q, q*d, d]) or 'listsf' (MHSA encoder over [q, d, q*d], then a univariate
+    FF net over [q, d, q*d, enc]; DivListNeuralRanker)."""
 
     def __init__(self, id='DiversityNeuralRanker', sf_para_dict=None, weight_decay=1e-3, gpu=False, device=None):
         self.sf_id = sf_para_dict['sf_id']
         assert self.sf_id in ['pointsf', 'listsf']
         if 'listsf' == self.sf_id:
-            raise NotImplementedError("the diversification list scorer (AttnDIN over [q, q*d, d]) is not implemented "
-                                      "yet; use sf_id='pointsf'")
+            check_listsf_config(sf_para_dict['listsf'])
         super().__init__(id=id, sf_para_dict=sf_para_dict, weight_decay=weight_decay, gpu=gpu, device=device)
-        # the scorer reads the concatenation [q, q*d, d] (diversity_ranker.py:22-23)
-        self.sf_para_dict[self.sf_id]['num_features'] *= 3
+        if 'pointsf' == self.sf_id:
+            # the scorer reads the concatenation [q, q*d, d] (diversity_ranker.py:22-23)
+            self.sf_para_dict[self.sf_id]['num_features'] *= 3
+        else:
+            # the list scorer widens its own layers (div_list_ranker.py:26); num_features stays F (diversity_ranker.py:24-25)
+            self.encoder_type = self.sf_para_dict['listsf']['encoder_type']
         self.queries_per_step = 1
+        self.attn_budget_bytes = ATTN_BUDGET_BYTES
         self._splits, self._weak_splits = {}, weakref.WeakKeyDictionary()
+
+    def init(self):
+        if 'pointsf' == self.sf_id:
+            return PointNeuralRanker.init(self)
+        self.list_sf = self.ini_listsf(**self.sf_para_dict['listsf'])
+        self.config_optimizer()
+
+    def get_parameters(self):
+        if 'pointsf' == self.sf_id:
+            return PointNeuralRanker.get_parameters(self)
+        return self.list_parameters()
 
     # ---- scorer ------------------------------------------------------------------------------------------------- #
     def ini_pointsf(self, num_features=None, h_dim=100, out_dim=1, num_layers=3, AF='R', TL_AF='S', apply_tl_af=False,
@@ -101,7 +131,9 @@ class DiversityNeuralRanker(PointNeuralRanker):
                             bn_per_query=bool(BN) and bn_type == 'BN')
 
     def div_forward(self, q_repr, doc_reprs):
-        """div_point_ranker.py:14-24: q_repr [1,F], doc_reprs [n,F] -> [1,n]."""
+        """div_point_ranker.py:14-24 / div_list_ranker.py:61-85: q_repr [1,F], doc_reprs [n,F] -> [1,n]."""
+        if 'listsf' == self.sf_id:
+            return self.list_div_forward(q_repr, doc_reprs)
         num_docs = doc_reprs.size(0)
         X = ops.div_features(q_repr.reshape(1, -1), doc_reprs.unsqueeze(0))
         return self.point_sf(X).view(-1, num_docs)
@@ -120,12 +152,12 @@ class DiversityNeuralRanker(PointNeuralRanker):
         try:
             sp = self._weak_splits.get(data)
             if sp is None:
-                sp = self._weak_splits[data] = _Split(data, self.device)
+                sp = self._weak_splits[data] = _Split(data, self.device, 'listsf' == self.sf_id)
             return sp
         except TypeError:                           # e.g. a plain list of query tuples
             hit = self._splits.get(id(data))
             if hit is None or hit[0] is not data:
-                hit = self._splits[id(data)] = (data, _Split(data, self.device))
+                hit = self._splits[id(data)] = (data, _Split(data, self.device, 'listsf' == self.sf_id))
             return hit[1]
 
     # ---- training ----------------------------------------------------------------------------------------------- #
@@ -135,7 +167,8 @@ class DiversityNeuralRanker(PointNeuralRanker):
         epoch ending at the first failing one.  ``queries_per_step`` (default: the ranker's ``queries_per_step``,
         1 = the reference) > 1 trains consecutive queries as one ragged batch: one scorer call with per-query BN
         statistics, one loss launch and one optimizer step on the sum of their losses.  The step losses are read back
-        once per epoch (the reference reads each with .item())."""
+        once per epoch (the reference reads each with .item()).  The list scorer runs the step's queries through the
+        encoder padded per length class, then uni_sf over their flat rows."""
         self.train_mode()
         qps = int(queries_per_step or self.queries_per_step)
         if qps < 1:
@@ -145,7 +178,13 @@ class DiversityNeuralRanker(PointNeuralRanker):
         losses, stop_training = [], False
         for q0, q1, r0, r1, off, max_len in sp.steps(qps):
             X = sp.X[r0:r1]
-            if q1 - q0 == 1:
+            if 'listsf' == self.sf_id:
+                batch_pred = self.list_scores(X, sp.plan(q0, q1, self))
+                if q1 - q0 == 1:
+                    batch_pred, layout = batch_pred.view(1, -1), {}
+                else:
+                    layout = dict(offsets=off, max_len=max_len)
+            elif q1 - q0 == 1:
                 batch_pred = self.point_sf(X.unsqueeze(0)).view(1, -1)
                 layout = {}
             else:
@@ -179,7 +218,10 @@ class DiversityNeuralRanker(PointNeuralRanker):
         self.eval_mode()
         sp = self._split(data)
         with torch.no_grad():
-            preds = self.div_forward_ragged(sp.X, sp.offsets, sp.max_len)
+            if 'listsf' == self.sf_id:
+                preds = self.list_scores(sp.X, sp.plan(0, len(sp), self))
+            else:
+                preds = self.div_forward_ragged(sp.X, sp.offsets, sp.max_len)
         res = ops.srd_metrics_at_ks(preds, sp.rele, ks, max_label=1.0 if max_label is None else max_label,
                                     offsets=sp.offsets, max_len=sp.max_len, return_order=return_order)
         return (sp, *res)
@@ -259,11 +301,37 @@ class DiversityNeuralRanker(PointNeuralRanker):
         else:
             raise NotImplementedError
 
-    # ---- checkpoints -------------------------------------------------------------------------------------------- #
+    # ---- modes and checkpoints ---------------------------------------------------------------------------------- #
+    def eval_mode(self):
+        if 'pointsf' == self.sf_id:
+            return PointNeuralRanker.eval_mode(self)
+        for part in self.list_sf.values():
+            part.eval()
+
+    def train_mode(self):
+        if 'pointsf' == self.sf_id:
+            return PointNeuralRanker.train_mode(self)
+        for part in self.list_sf.values():
+            part.train(mode=True)
+
+    def save(self, dir, name):
+        """pointsf: the scorer's state_dict; listsf: {'encoder': ..., 'uni_sf': ...} (div_list_ranker.py:100-105)."""
+        if 'pointsf' == self.sf_id:
+            return PointNeuralRanker.save(self, dir, name)
+        if not os.path.exists(dir):
+            os.makedirs(dir)
+        torch.save({'encoder': self.list_sf['encoder'].state_dict(), 'uni_sf': self.list_sf['uni_sf'].state_dict()},
+                   dir + name)
+
     def load(self, file_model, **kwargs):
         """The driver loads with context='cpu_gpu' and no device (ltr_diversification.py:296-302)."""
         device = kwargs.get('device') or self.device
-        self.point_sf.load_state_dict(torch.load(file_model, map_location=device))
+        if 'pointsf' == self.sf_id:
+            self.point_sf.load_state_dict(torch.load(file_model, map_location=device))
+            return
+        checkpoint = torch.load(file_model, map_location=device)
+        self.list_sf['encoder'].load_state_dict(checkpoint['encoder'])
+        self.list_sf['uni_sf'].load_state_dict(checkpoint['uni_sf'])
 
     def uniform_eval_setting(self, **kwargs):
         pass

@@ -644,6 +644,102 @@ def div_features(q_repr: torch.Tensor, docs: torch.Tensor, offsets: Optional[tor
     return out
 
 
+@_on_tensor_device
+def div_list_features(q_repr: torch.Tensor, docs: torch.Tensor, offsets: Optional[torch.Tensor] = None,
+                      max_len: Optional[int] = None) -> torch.Tensor:
+    """[q, d, q*d] rows, the encoder input of the diversification list scorer (div_list_ranker.py:61-64; d comes before
+    q*d here, unlike :func:`div_features`).  Layouts as :func:`div_features`; forward only."""
+    lib = _lib.load()
+    q, d = _dev_f32(q_repr, "q_repr"), _dev_f32(docs, "docs")
+    F = d.shape[-1]
+    if offsets is None:
+        if d.dim() != 3:
+            raise ValueError(f"expected [B,n,F] documents, got {tuple(d.shape)}")
+        B, n, op = d.shape[0], d.shape[1], None
+    else:
+        if d.dim() != 2 or max_len is None:
+            raise ValueError("ragged documents are [total_docs, F] with offsets= and max_len=")
+        offsets = offsets.to(device=d.device, dtype=torch.int32).contiguous()
+        B, n, op = offsets.numel() - 1, max(int(max_len), 1), offsets.data_ptr()
+    if q.shape != (B, F):
+        raise ValueError(f"q_repr {tuple(q.shape)} does not match {B} queries of width {F}")
+    out = torch.empty((*d.shape[:-1], 3 * F), dtype=torch.float32, device=d.device)
+    if d.numel():
+        _lib.check(lib.ptrb200_div_list_features(q.data_ptr(), d.data_ptr(), op, out.data_ptr(), B, n, F, _stream_ptr()),
+                   "div_list_features")
+    return out
+
+
+def _class_ptrs(offsets: torch.Tensor, qidx: torch.Tensor, device):
+    for t, name in ((offsets, "offsets"), (qidx, "qidx")):
+        if t.device != device or t.dtype != torch.int32 or not t.is_contiguous():
+            raise ValueError(f"{name} must be a contiguous int32 tensor on {device}")
+    return offsets.data_ptr(), qidx.data_ptr()
+
+
+@_on_tensor_device
+def pad_lists_pitched(src: torch.Tensor, offsets: torch.Tensor, qidx: torch.Tensor, n_max: int,
+                      col0: int = 0, width: Optional[int] = None) -> torch.Tensor:
+    """Columns [col0, col0 + width) of the ragged rows ``src`` [total, C] for the queries ``qidx`` (int32, indices into
+    the prefix ``offsets``) -> dense [len(qidx), n_max, width], zero behind each list.  Forward only."""
+    lib = _lib.load()
+    src = _dev_f32(src, "src")
+    if src.dim() != 2:
+        raise ValueError("src must be [total, C]")
+    width = src.shape[1] - col0 if width is None else int(width)
+    if col0 < 0 or width <= 0 or col0 + width > src.shape[1]:
+        raise ValueError(f"columns [{col0}, {col0 + width}) outside a row of {src.shape[1]}")
+    op, qp = _class_ptrs(offsets, qidx, src.device)
+    out = torch.empty((qidx.numel(), int(n_max), width), dtype=torch.float32, device=src.device)
+    _lib.check(lib.ptrb200_pad_lists_pitched(src.data_ptr() + 4 * col0, src.shape[1], op, qp, out.data_ptr(), qidx.numel(),
+                                             int(n_max), width, _stream_ptr()), "pad_lists_pitched")
+    return out
+
+
+class _DivListConcat(torch.autograd.Function):
+    """[feats | unpadded encoder output] rows, the uni_sf input (div_list_ranker.py:80).  Every length class's launch
+    writes both halves of its rows; backward pads columns [W, 2W) of the gradient back into each class's padded layout
+    (zeros behind each list).  ``feats`` is data: it gets no gradient."""
+
+    @staticmethod
+    @_on_tensor_device
+    def forward(ctx, feats, offsets, qidxs, *blocks):
+        lib = _lib.load()
+        feats = _dev_f32(feats, "feats")
+        W = feats.shape[1]
+        out = torch.empty((feats.shape[0], 2 * W), dtype=torch.float32, device=feats.device)
+        for qidx, enc in zip(qidxs, blocks):
+            enc = _dev_f32(enc, "enc")
+            if enc.dim() != 3 or enc.shape[0] != qidx.numel() or enc.shape[2] != W:
+                raise ValueError(f"encoder block {tuple(enc.shape)} does not match {qidx.numel()} queries of width {W}")
+            op, qp = _class_ptrs(offsets, qidx, feats.device)
+            _lib.check(lib.ptrb200_div_list_concat(feats.data_ptr(), enc.data_ptr(), op, qp, out.data_ptr(), qidx.numel(),
+                                                   enc.shape[1], W, _stream_ptr()), "div_list_concat")
+        ctx.save_for_backward(offsets, *qidxs)
+        ctx.n_maxs = [b.shape[1] for b in blocks]
+        return out
+
+    @staticmethod
+    @_on_tensor_device
+    def backward(ctx, g):
+        offsets, *qidxs = ctx.saved_tensors
+        g = _dev_f32(g, "g")
+        W = g.shape[1] // 2
+        return (None, None, None,
+                *[pad_lists_pitched(g, offsets, q, n, col0=W, width=W) for q, n in zip(qidxs, ctx.n_maxs)])
+
+
+def div_list_concat(feats: torch.Tensor, offsets: torch.Tensor, qidxs: Sequence[torch.Tensor],
+                    blocks: Sequence[torch.Tensor]) -> torch.Tensor:
+    """feats [rows, W] + padded encoder outputs ``blocks[c]`` [len(qidxs[c]), n_c, W] of length classes that together
+    cover every non-empty query of ``offsets`` once -> [rows, 2W] (differentiable in the blocks)."""
+    if not blocks or len(blocks) != len(qidxs):
+        raise ValueError("one encoder block per length class")
+    if sum(int(q.numel()) for q in qidxs) > offsets.numel() - 1:
+        raise ValueError("the length classes must cover every query at most once")
+    return _DivListConcat.apply(feats, offsets, list(qidxs), *blocks)
+
+
 # --------------------------------------------------------------------------- #
 # stacked feed-forward scorer
 # --------------------------------------------------------------------------- #

@@ -10,7 +10,8 @@ The reference is imported from baseline/_ref (a pip --target install of wildltr/
 the checkout named by PTRANKING_REFERENCE.  Data: a synthetic data directory in the TREC Web-track diversification
 layout the driver reads (load_raw_data, :155-207) -- query_permutation.json, query_representation.dat,
 doc_representation.dat, query_doc.json and folder{1..5}/config.yml -- with 100-dimensional representations and
-documents covering 1 to 6 subtopics.  debug=True (5 folds, alpha-nDCG@5 validation), 2 epochs, default pointsf.
+documents covering 1 to 6 subtopics.  debug=True (5 folds, alpha-nDCG@5 validation), 2 epochs, the pointsf scorer
+by default; ``--sf listsf`` runs the list scorer with the reference's default listsf dict (div_parameter.py:98-104).
 """
 import argparse
 import json
@@ -82,6 +83,7 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--cuda", default="0")
     ap.add_argument("--keep", action="store_true")
+    ap.add_argument("--sf", default="pointsf", choices=["pointsf", "listsf"])
     args = ap.parse_args()
 
     work = tempfile.mkdtemp(prefix="div_dropin_")
@@ -94,7 +96,7 @@ def main():
     import torch
     import ptranking.ltr_diversification.eval.ltr_diversification as ref_div
     from ptranking.ltr_diversification.eval.div_parameter import DivEvalSetting
-    print(f"reference imported from {REF}; impl = {args.impl}; model = DALETOR; scorer = pointsf")
+    print(f"reference imported from {REF}; impl = {args.impl}; model = DALETOR; scorer = {args.sf}")
     if args.impl == "b200":
         import ptranking_b200
         ptranking_b200.install_diversification()
@@ -114,7 +116,7 @@ def main():
     cuda = None if args.cuda == "none" else int(args.cuda)
     evaluator = ref_div.DivLTREvaluator(cuda=cuda)
     t0 = time.time()
-    evaluator.run(debug=True, model_id="DALETOR", sf_id="pointsf", data_id="WT_Div_0912_Implicit", dir_data=data_dir,
+    evaluator.run(debug=True, model_id="DALETOR", sf_id=args.sf, data_id="WT_Div_0912_Implicit", dir_data=data_dir,
                   dir_output=out_dir)
     dt = time.time() - t0
     print(f"DivLTREvaluator.run finished in {dt:.1f} s (5 folds x {EPOCHS} epochs)")
