@@ -392,14 +392,18 @@ __global__ void __launch_bounds__(RG_THREADS) rows_gemm_tc_kernel(RowsGemmArgs g
 //   warps 8-15  producers: global -> registers (prefetched one chunk ahead) -> prologue -> hi/lo split ->
 //                          swizzled A stage (ring of 2)
 // Producers and consumers only meet through mbarriers (aready/afree per A stage): the producers stage tile t+1
-// while the consumers multiply and write out tile t.  512 threads leave 128 registers per thread, room for a
-// 64 x 128 accumulator per consumer thread and the producers' four prefetched units.
+// while the consumers multiply and write out tile t.  512 threads start with 128 registers each; after the role
+// branch the consumers give theirs down to RW_CONS_REGS (a 64 x 128 accumulator, descriptors, epilogue) and the
+// producers take RW_PROD_REGS (the staged and the prefetched chunk, per-tile pointers, dropout keys): at 128 each
+// the producers spill.
 // --------------------------------------------------------------------------------------------
 constexpr int RW_EPI_WARPS = 8, RW_PROD_WARPS = 8;
 constexpr int RW_THREADS = (RW_EPI_WARPS + RW_PROD_WARPS) * 32;
 constexpr int RW_PRODUCERS = RW_PROD_WARPS * 32;
 constexpr int RW_PU = 128 * 8 / RW_PRODUCERS;            // 16-byte A units per producer thread per chunk
 constexpr int RW_MAX_N = 128;
+constexpr int RW_CONS_REGS = 120, RW_PROD_REGS = 136;
+static_assert((RW_CONS_REGS * RW_EPI_WARPS + RW_PROD_REGS * RW_PROD_WARPS) * 32 <= 65536, "register split exceeds the register file");
 
 struct RowsWsExtra {
     int ntiles;
@@ -450,6 +454,7 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
     const int my_tiles = blockIdx.x < x.ntiles ? (x.ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
 
     if (warp >= RW_EPI_WARPS) {
+        tc::setmaxnreg_inc<RW_PROD_REGS>();
         if constexpr (MODE == RG_DGRAD) {
         // (the data-gradient instantiation keeps the simpler producer loop: its fused dZ = k1*dY + k3*Z + k0 staging carries
         //  more live state, and the restructured loop below would add to it)
@@ -704,7 +709,9 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
                 }
             }
         }
-    } else if (my_tiles > 0) {
+    } else {
+        tc::setmaxnreg_dec<RW_CONS_REGS>();
+        if (my_tiles > 0) {
         // ================================ consumer warps (0..7) ================================
         // warpgroup wg multiplies rows [64 wg, +64) of every tile; the accumulator of the tile stays in registers
         const int wg = warp >> 2;
@@ -732,9 +739,12 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
             for (int c = 0; c < nchunks; ++c, ++q) {
                 const int s = q & 1;
                 tc::mbar_wait(aready + s, (q >> 1) & 1);
-                const uint32_t a_addr = a_base + s * 32768;
+                uint32_t a_addr = a_base + s * 32768, b_off = c * wchunk;
+                // opaque to the optimiser: the descriptors are rebuilt at every chunk (a few integer ops) instead of being
+                // hoisted out of the tile loop, where the unrolled chunks' descriptors outgrow the consumers' registers
+                asm volatile("" : "+r"(a_addr), "+r"(b_off));
                 const uint64_t ah = tc::smem_desc_sw128(a_addr, 1024), al = tc::smem_desc_sw128(a_addr + 16384, 1024);
-                const uint64_t bh = tc::smem_desc_sw128(wh_base + c * wchunk, 1024), bl = tc::smem_desc_sw128(wl_base + c * wchunk, 1024);
+                const uint64_t bh = tc::smem_desc_sw128(wh_base + b_off, 1024), bl = tc::smem_desc_sw128(wl_base + b_off, 1024);
                 // four K-steps per chunk (+32 B along K inside the swizzle atom each; columns beyond K are staged as zeros)
                 tc::wg_fence();
 #pragma unroll
@@ -754,6 +764,8 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
             __syncwarp();
             if (lane == 0) tc::mbar_arrive(afree + ((q - 1) & 1));
             // ---- epilogue: registers -> (+bias | dropout mask) -> global rows, per-warp column sums ----
+            const float* bias = g.bias;
+            asm volatile("" : "+l"(bias));          // loaded per tile: hoisted over the tile loop the bias would hold NPc / 2 registers
             bool live[2];
             float* orow[2];
 #pragma unroll
@@ -766,7 +778,7 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
             for (int e = 0; e < NPc / 2; ++e) {
                 const int col = tc::acc_col(e);
                 if (col >= N) { acc[e] = 0.0f; continue; }
-                if (MODE == RG_FWD) acc[e] += __ldg(g.bias + col);
+                if (MODE == RG_FWD) acc[e] += __ldg(bias + col);
                 else if (g.drop.thr) {
                     const int r = wg * 64 + tc::acc_row(e);
                     acc[e] = dropout_keep(g.drop.key, (uint64_t)(row0 + r) * N + col, g.drop.thr) ? acc[e] * g.drop.scale : 0.0f;
@@ -781,6 +793,8 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
                 else { orow[h][col] = acc[e]; if (col + 1 < N) orow[h][col + 1] = acc[e + 1]; }
             }
             if (MODE == RG_FWD && x.stats_mode) {
+                int sl = lane, sw = warp;
+                asm volatile("" : "+r"(sl), "+r"(sw));  // per tile, like the bias: the NPc / 4 stat_sm offsets are not kept live
 #pragma unroll
                 for (int j = 0; j < NPc / 16; ++j) {
                     const float* w = acc + 8 * j;
@@ -799,12 +813,12 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
                             s1[p] += __shfl_xor_sync(0xffffffffu, s1[p], o);
                             s2[p] += __shfl_xor_sync(0xffffffffu, s2[p], o);
                         }
-                    if (lane < 4) {
+                    if (sl < 4) {
 #pragma unroll
                         for (int p = 0; p < 4; ++p) {
-                            const int col = j * 16 + (p >> 1) * 8 + 2 * lane + (p & 1);
-                            stat_sm[(warp * NP + col) * 2] = s1[p];
-                            stat_sm[(warp * NP + col) * 2 + 1] = s2[p];
+                            const int col = j * 16 + (p >> 1) * 8 + 2 * sl + (p & 1);
+                            stat_sm[(sw * NP + col) * 2] = s1[p];
+                            stat_sm[(sw * NP + col) * 2 + 1] = s2[p];
                         }
                     }
                 }
@@ -826,9 +840,10 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
             double* p = g.partials + ((size_t)blockIdx.x * N + tid) * 2;
             p[0] = acc1; p[1] = acc2;
         }
-    } else if (MODE == RG_FWD && x.stats_mode == 1 && tid < N) {      // a CTA without tiles contributes zero sums
-        double* p = g.partials + ((size_t)blockIdx.x * N + tid) * 2;
-        p[0] = 0.0; p[1] = 0.0;
+        } else if (MODE == RG_FWD && x.stats_mode == 1 && tid < N) {      // a CTA without tiles contributes zero sums
+            double* p = g.partials + ((size_t)blockIdx.x * N + tid) * 2;
+            p[0] = 0.0; p[1] = 0.0;
+        }
     }
 }
 
