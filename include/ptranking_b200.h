@@ -428,19 +428,11 @@ int ptrb200_rmsprop_step_peer(const ptrb200_peer_group* grp, float* param, float
 
 /* ---- multi-head self-attention list scorer ------------------------------------------------ */
 /* MultiheadAttention.forward, ptranking/base/list_ranker.py:226-248: for every (query b, head h)
- * O = dropout(softmax(Q K^T / sqrt(D))) V, flash-style (no [n,n] tensor in HBM).  Q,K,V,O: [B,n,H*D] with head h
- * in columns [h*D,(h+1)*D) (the reference's view/permute, :222-224, :251).  LSE[B,H,n] is kept for backward. */
-int ptrb200_attention_fwd(const float* Q, const float* K, const float* V, float* O, float* LSE,
-                          int B, int n, int H, int D, float dropout_p, uint64_t seed, uint64_t offset,
-                          ptrb200_stream_t stream);
-/* autograd of the above; scratch: B*H*n floats. */
-int ptrb200_attention_bwd(const float* Q, const float* K, const float* V, const float* O, const float* dO, const float* LSE,
-                          float* dQ, float* dK, float* dV, float* scratch,
-                          int B, int n, int H, int D, float dropout_p, uint64_t seed, uint64_t offset,
-                          ptrb200_stream_t stream);
-/* Tensor-core variant of the two calls above (same maths, same dropout stream): every contraction is a batched
- * wgmma tf32 GEMM (passes = 3: 3xTF32 split, fp32-grade; 1: plain TF32); the attention matrix
- * P[B*H,n,n] is materialised in HBM and kept for the backward pass.
+ * O = dropout(softmax(Q K^T / sqrt(D))) V.  Q,K,V,O: [B,n,H*D] with head h in columns [h*D,(h+1)*D) (the reference's
+ * view/permute, :222-224, :251).  Every contraction is a batched wgmma GEMM in 3xTF32 (split operands, fp32-grade
+ * results); `passes` must be 3, any other value returns PTRB200_ERR_UNSUPPORTED.  The attention matrix P[B*H,n,n]
+ * is materialised in HBM and kept for the backward pass.  Dropout keeps element ((b*H+h)*n + i)*n + j of P with the
+ * stream of PTRB200_EW_DROPOUT over a flat [B*H,n,n] tensor.
  * scratch: ptrb200_attention_tc_workspace_floats(B,n,H,D,backward) floats. */
 int64_t ptrb200_attention_tc_workspace_floats(int B, int n, int H, int D, int backward);
 int ptrb200_attention_tc_fwd(const float* Q, const float* K, const float* V, float* O, float* P_out, float* scratch,

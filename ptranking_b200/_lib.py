@@ -87,7 +87,6 @@ SIGNATURES = {
     "ptrb200_sum_f32": (_I, [_fp, _fp, _I, _fp]),
     "ptrb200_ndcg_at_ks": (_I, [_fp, _fp, _fp, C.POINTER(C.c_int32), _I, _fp, _fp, _I, _I, _I, _fp]),
     "ptrb200_adhoc_metrics_at_ks": (_I, [_fp, _fp, _fp, C.POINTER(C.c_int32), _I, _fp, _I, _I, _I, _F, _fp]),
-    "ptrb200_attention_fwd": (_I, [_fp, _fp, _fp, _fp, _fp, _I, _I, _I, _I, _F, _U64, _U64, _fp]),
     "ptrb200_adam_step": (_I, [_fp, _fp, _fp, _fp, _I64, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, _I, _fp]),
     "ptrb200_adagrad_step": (_I, [_fp, _fp, _fp, _I64, C.c_double, C.c_double, C.c_double, C.c_double, _I, _fp]),
     "ptrb200_rmsprop_step": (_I, [_fp, _fp, _fp, _I64, C.c_double, C.c_double, C.c_double, C.c_double, _fp]),
@@ -98,7 +97,6 @@ SIGNATURES = {
     "ptrb200_pad_lists": (_I, [_fp, _fp, _fp, _I, _I, _I, _fp]),
     "ptrb200_unpad_lists": (_I, [_fp, _fp, _fp, _I, _I, _I, _fp]),
     "ptrb200_attention_tc_bwd_ld": (_I, [_fp] * 9 + [_I, _I, _I, _I, _I, _I, _F, _U64, _U64, _I, _fp]),
-    "ptrb200_attention_bwd": (_I, [_fp] * 10 + [_I, _I, _I, _I, _F, _U64, _U64, _fp]),
     "ptrb200_layernorm_fwd": (_I, [_fp, _fp, _fp, _fp, _fp, _fp, _I, _I, _F, _fp]),
     "ptrb200_layernorm_bwd": (_I, [_fp] * 9 + [_I, _I, _F, _fp]),
     "ptrb200_elementwise": (_I, [_I, _fp, _fp, _fp, _I64, _F, _U64, _U64, _fp]),

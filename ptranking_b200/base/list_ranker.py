@@ -49,18 +49,12 @@ class MultiheadAttention(nn.Module):
 
     def forward(self, x):
         p = self.p if self.training else 0.0
-        if ops.attention_impl() in ("tc", "tc_tf32") and os.environ.get("PTRANKING_B200_FUSED_QKV", "1") == "1":
-            # Q|K|V = x [Wq;Wk;Wv]^T + [bq;bk;bv]: one hid -> 3*hid contraction (column for column the reference's three,
-            # list_ranker.py:233-235), read in place by the attention kernels; its backward is one data-gradient and
-            # one weight-gradient contraction instead of three each plus two tensor additions
-            W = ops.adjacent_rows(self.w_q.weight, self.w_k.weight, self.w_v.weight)
-            b = ops.adjacent_rows(self.w_q.bias, self.w_k.bias, self.w_v.bias)
-            ctx = ops.attention_packed(ops.linear(x, W, b), self.n_heads, p)
-        else:
-            Q = ops.linear(x, self.w_q.weight, self.w_q.bias)
-            K = ops.linear(x, self.w_k.weight, self.w_k.bias)
-            V = ops.linear(x, self.w_v.weight, self.w_v.bias)
-            ctx = ops.attention(Q, K, V, self.n_heads, p)
+        # Q|K|V = x [Wq;Wk;Wv]^T + [bq;bk;bv]: one hid -> 3*hid contraction (column for column the reference's three,
+        # list_ranker.py:233-235), read in place by the attention kernels; its backward is one data-gradient and
+        # one weight-gradient contraction instead of three each plus two tensor additions
+        W = ops.adjacent_rows(self.w_q.weight, self.w_k.weight, self.w_v.weight)
+        b = ops.adjacent_rows(self.w_q.bias, self.w_k.bias, self.w_v.bias)
+        ctx = ops.attention_packed(ops.linear(x, W, b), self.n_heads, p)
         return ops.linear(ctx, self.fc.weight, self.fc.bias)
 
 

@@ -54,7 +54,7 @@ static __device__ __forceinline__ void store_op(unsigned char* buf, bool mn, uin
 // the four K-steps of one 32-column chunk (columns beyond K are staged as zeros): warpgroup wg multiplies A rows
 // [64 wg, +64) by all NPc columns of B.  3xTF32: the small a_lo*b_hi + a_hi*b_lo terms accumulate apart from the main
 // products (the epilogue adds them), so two thirds of the accumulate steps leave the main chain.
-template <int PASSES, int NPc>
+template <int NPc>
 static __device__ __forceinline__ void bg_mma_chunk(float (&acc)[NPc / 2], float (&cor)[NPc / 2], const unsigned char* a_hi,
                                                     const unsigned char* b_hi, int wg) {
     const uint32_t a_s = tc::smem_u32(a_hi) + wg * 8192, b_s = tc::smem_u32(b_hi);
@@ -63,17 +63,14 @@ static __device__ __forceinline__ void bg_mma_chunk(float (&acc)[NPc / 2], float
     tc::wg_fence();
 #pragma unroll
     for (int s = 0; s < 4; ++s) {
-        if (PASSES == 3) {
-            tc::mma_tf32<NPc>(cor, al + 2 * s, bh + 2 * s, 1u);
-            tc::mma_tf32<NPc>(cor, ah + 2 * s, bl + 2 * s, 1u);
-        }
+        tc::mma_tf32<NPc>(cor, al + 2 * s, bh + 2 * s, 1u);
+        tc::mma_tf32<NPc>(cor, ah + 2 * s, bl + 2 * s, 1u);
         tc::mma_tf32<NPc>(acc, ah + 2 * s, bh + 2 * s, 1u);
     }
     tc::wg_commit();
     tc::wg_wait<0>();                 // the same threads stage the next chunk
 }
 
-template <int PASSES>
 __global__ void __launch_bounds__(BG_THREADS) bgemm_nt_tc_kernel(BGemmArgs g) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -148,16 +145,16 @@ __global__ void __launch_bounds__(BG_THREADS) bgemm_nt_tc_kernel(BGemmArgs g) {
             }
             float4 h, l;
             tc::split_tf32_rn(v.x, h.x, l.x); tc::split_tf32_rn(v.y, h.y, l.y); tc::split_tf32_rn(v.z, h.z, l.z); tc::split_tf32_rn(v.w, h.w, l.w);
-            store_op(a_hi, g.a_mn, off_k, mu, kr, PASSES == 3 ? h : v);
-            if (PASSES == 3) store_op(a_lo, g.a_mn, off_k, mu, kr, l);
+            store_op(a_hi, g.a_mn, off_k, mu, kr, h);
+            store_op(a_lo, g.a_mn, off_k, mu, kr, l);
             const float4 w = bv[i];
             tc::split_tf32_rn(w.x, h.x, l.x); tc::split_tf32_rn(w.y, h.y, l.y); tc::split_tf32_rn(w.z, h.z, l.z); tc::split_tf32_rn(w.w, h.w, l.w);
-            store_op(b_hi, g.b_mn, off_k, mu, kr, PASSES == 3 ? h : w);
-            if (PASSES == 3) store_op(b_lo, g.b_mn, off_k, mu, kr, l);
+            store_op(b_hi, g.b_mn, off_k, mu, kr, h);
+            store_op(b_lo, g.b_mn, off_k, mu, kr, l);
         }
         tc::fence_proxy_async();
         __syncthreads();
-        bg_mma_chunk<PASSES, NPc>(acc, cor, a_hi, b_hi, wg);
+        bg_mma_chunk<NPc>(acc, cor, a_hi, b_hi, wg);
     }
     {   // epilogue: registers -> C
         const bool vecC = (g.ldc & 3) == 0 && ((reinterpret_cast<uintptr_t>(C + n0) & 15) == 0);
@@ -181,7 +178,7 @@ __global__ void __launch_bounds__(BG_THREADS) bgemm_nt_tc_kernel(BGemmArgs g) {
 // chunk loop; one 64-bit draw serves the four elements of a unit (the general kernel hashes per element because it
 // cannot assume quad alignment); B units beyond the padded tile width are never touched.  The attention core's six
 // contractions all qualify; odd shapes keep the general kernel.
-template <int PASSES, int A_MN, int B_MN, int DROP>
+template <int A_MN, int B_MN, int DROP>
 __global__ void __launch_bounds__(BG_THREADS, 1) bgemm_fast_kernel(BGemmArgs g) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -282,19 +279,19 @@ __global__ void __launch_bounds__(BG_THREADS, 1) bgemm_fast_kernel(BGemmArgs g) 
             }
             float4 h, l;
             tc::split_tf32_rn(v.x, h.x, l.x); tc::split_tf32_rn(v.y, h.y, l.y); tc::split_tf32_rn(v.z, h.z, l.z); tc::split_tf32_rn(v.w, h.w, l.w);
-            put(a_hi, A_MN, oa, i, PASSES == 3 ? h : v);
-            if (PASSES == 3) put(a_lo, A_MN, oa, i, l);
+            put(a_hi, A_MN, oa, i, h);
+            put(a_lo, A_MN, oa, i, l);
             if ((bm >> (4 + i)) & 1u) {
                 const float4 w = bv[i];
                 tc::split_tf32_rn(w.x, h.x, l.x); tc::split_tf32_rn(w.y, h.y, l.y); tc::split_tf32_rn(w.z, h.z, l.z); tc::split_tf32_rn(w.w, h.w, l.w);
-                put(b_hi, B_MN, ob, i, PASSES == 3 ? h : w);
-                if (PASSES == 3) put(b_lo, B_MN, ob, i, l);
+                put(b_hi, B_MN, ob, i, h);
+                put(b_lo, B_MN, ob, i, l);
             }
         }
         dctr += dstep_c;
         tc::fence_proxy_async();
         __syncthreads();
-        bg_mma_chunk<PASSES, NPc>(acc, cor, a_hi, b_hi, wg);
+        bg_mma_chunk<NPc>(acc, cor, a_hi, b_hi, wg);
     }
     const float alpha = g.alpha;
     if (N == BG_NT) {
@@ -325,11 +322,11 @@ __global__ void __launch_bounds__(BG_THREADS, 1) bgemm_fast_kernel(BGemmArgs g) 
     });
 }
 
-// in-place row softmax over S[z][i][:] (one warp per row); also emits the per-row log-sum-exp.
+// in-place row softmax over S[z][i][:] (one warp per row).
 // key_lens (optional, [B]): only the first key_lens[b] keys of query b exist (a ragged batch padded to n); the others get
 // probability exactly 0, so padded documents influence nothing (their own rows are never read back).
-__global__ void softmax_rows_kernel(float* __restrict__ S, float* __restrict__ lse, size_t rows, int n,
-                                    const int32_t* __restrict__ key_lens, int rows_per_query) {
+__global__ void softmax_rows_kernel(float* __restrict__ S, size_t rows, int n, const int32_t* __restrict__ key_lens,
+                                    int rows_per_query) {
     const size_t row = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (row >= rows) return;
@@ -344,7 +341,6 @@ __global__ void softmax_rows_kernel(float* __restrict__ S, float* __restrict__ l
     const float inv = 1.0f / l;
     for (int j = lane; j < nk; j += 32) s[j] *= inv;
     for (int j = nk + lane; j < n; j += 32) s[j] = 0.0f;
-    if (lane == 0 && lse) lse[row] = m + logf(l);
 }
 
 // dS = A * (dA - sum_j A dA) * inv_scale in place over dAd, where dA = dropmask(dAd)  (one warp per row)
@@ -366,11 +362,11 @@ __global__ void softmax_bwd_rows_kernel(const float* __restrict__ P, float* __re
     for (int j = lane; j < n; j += 32) d[j] = p[j] * (d[j] - acc) * inv_scale;
 }
 
-template <int PASSES, int A_MN, int B_MN, int DROP>
+template <int A_MN, int B_MN, int DROP>
 static int launch_bgemm_fast(const BGemmArgs& g, dim3 grid, size_t smem, cudaStream_t st, const char* tag) {
-    const cudaError_t e = cudaFuncSetAttribute(bgemm_fast_kernel<PASSES, A_MN, B_MN, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const cudaError_t e = cudaFuncSetAttribute(bgemm_fast_kernel<A_MN, B_MN, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { set_error("bgemm smem attr: %s", cudaGetErrorString(e)); return PTRB200_ERR_CUDA; }
-    PTRB200_LAUNCH_TAG(tag, (bgemm_fast_kernel<PASSES, A_MN, B_MN, DROP>), grid, BG_THREADS, smem, st, g);
+    PTRB200_LAUNCH_TAG(tag, (bgemm_fast_kernel<A_MN, B_MN, DROP>), grid, BG_THREADS, smem, st, g);
     return PTRB200_OK;
 }
 
@@ -379,7 +375,7 @@ static bool bgemm_general_forced() {
     return e && e[0] == '1';
 }
 
-static int launch_bgemm(BGemmArgs& g, int Z, int passes, cudaStream_t st, const char* tag) {
+static int launch_bgemm(BGemmArgs& g, int Z, cudaStream_t st, const char* tag) {
     const size_t smem = 1024 + 4 * 16384;
     dim3 grid((g.M + 127) / 128, (g.N + BG_NT - 1) / BG_NT, Z);
     // the alignment-specialised kernel: every pitch, stride, extent and base address a multiple of four floats
@@ -391,22 +387,14 @@ static int launch_bgemm(BGemmArgs& g, int Z, int passes, cudaStream_t st, const 
     if (fast) {
         const int drop = g.drop.thr ? g.drop_mode : 0;
         const size_t smem = 1024 + (size_t)128 * (BG_NT + 4) * 4;      // operands (64 KB) overlaid by the [128][132] output staging tile
-#define PTRB200_BG_CASE(P, AM, BM, D) if ((passes == 3) == (P == 3) && g.a_mn == AM && g.b_mn == BM && drop == D) return launch_bgemm_fast<P, AM, BM, D>(g, grid, smem, st, tag);
-        // the attention core's shapes (list_ranker.py:226-248 forward + autograd), 3xTF32 and single-pass
-        PTRB200_BG_CASE(3, 0, 0, 0) PTRB200_BG_CASE(3, 0, 1, 0) PTRB200_BG_CASE(3, 0, 1, 1) PTRB200_BG_CASE(3, 1, 1, 0) PTRB200_BG_CASE(3, 1, 1, 2)
-        PTRB200_BG_CASE(1, 0, 0, 0) PTRB200_BG_CASE(1, 0, 1, 0) PTRB200_BG_CASE(1, 0, 1, 1) PTRB200_BG_CASE(1, 1, 1, 0) PTRB200_BG_CASE(1, 1, 1, 2)
+#define PTRB200_BG_CASE(AM, BM, D) if (g.a_mn == AM && g.b_mn == BM && drop == D) return launch_bgemm_fast<AM, BM, D>(g, grid, smem, st, tag);
+        // the attention core's shapes (list_ranker.py:226-248 forward + autograd)
+        PTRB200_BG_CASE(0, 0, 0) PTRB200_BG_CASE(0, 1, 0) PTRB200_BG_CASE(0, 1, 1) PTRB200_BG_CASE(1, 1, 0) PTRB200_BG_CASE(1, 1, 2)
 #undef PTRB200_BG_CASE
     }
-    cudaError_t e;
-    if (passes == 3) {
-        e = cudaFuncSetAttribute(bgemm_nt_tc_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) { set_error("bgemm smem attr: %s", cudaGetErrorString(e)); return PTRB200_ERR_CUDA; }
-        PTRB200_LAUNCH_TAG(tag, bgemm_nt_tc_kernel<3>, grid, BG_THREADS, smem, st, g);
-    } else {
-        e = cudaFuncSetAttribute(bgemm_nt_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) { set_error("bgemm smem attr: %s", cudaGetErrorString(e)); return PTRB200_ERR_CUDA; }
-        PTRB200_LAUNCH_TAG(tag, bgemm_nt_tc_kernel<1>, grid, BG_THREADS, smem, st, g);
-    }
+    const cudaError_t e = cudaFuncSetAttribute(bgemm_nt_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) { set_error("bgemm smem attr: %s", cudaGetErrorString(e)); return PTRB200_ERR_CUDA; }
+    PTRB200_LAUNCH_TAG(tag, bgemm_nt_tc_kernel, grid, BG_THREADS, smem, st, g);
     return PTRB200_OK;
 }
 
@@ -428,6 +416,7 @@ int ptrb200_attention_tc_fwd_ld(const float* Q, const float* K, const float* V, 
                                 int B, int n, int H, int D, int ld_qkv, int ld_o, const int32_t* key_lens, float dropout_p,
                                 uint64_t seed, uint64_t offset, int passes, ptrb200_stream_t stream) {
     if (!Q || !K || !V || !O || !P_out || !scratch || B <= 0 || n <= 0 || H <= 0 || D <= 0) { set_error("attention_tc_fwd: bad arguments"); return PTRB200_ERR_INVALID; }
+    if (passes != 3) { set_error("attention_tc_fwd: passes must be 3 (3xTF32), got %d", passes); return PTRB200_ERR_UNSUPPORTED; }
     cudaStream_t st = (cudaStream_t)stream;
     const int Z = B * H, HD = H * D;
     const int lq = ld_qkv > 0 ? ld_qkv : HD, lo = ld_o > 0 ? ld_o : HD;
@@ -438,16 +427,16 @@ int ptrb200_attention_tc_fwd_ld(const float* Q, const float* K, const float* V, 
     // S = Q K^T / sqrt(D)
     g.A = Q; g.B = K; g.C = P_out; g.M = n; g.N = n; g.K = D; g.lda = lq; g.ldb = lq; g.ldc = n;
     g.sAb = sb; g.sAh = sh; g.sBb = sb; g.sBh = sh; g.sCb = nn * H; g.sCh = nn; g.H = H; g.alpha = 1.0f / sqrtf((float)D);
-    if ((rc = launch_bgemm(g, Z, passes, st, "attn_tc_qk"))) return rc;
+    if ((rc = launch_bgemm(g, Z, st, "attn_tc_qk"))) return rc;
     const size_t rows = (size_t)Z * n;
-    PTRB200_LAUNCH(softmax_rows_kernel, (unsigned)((rows + 7) / 8), 256, 0, st, P_out, (float*)nullptr, rows, n, key_lens, H * n);
+    PTRB200_LAUNCH(softmax_rows_kernel, (unsigned)((rows + 7) / 8), 256, 0, st, P_out, rows, n, key_lens, H * n);
     // O = dropout(P) V : V is the [K = key, N = d] row-major factor, consumed MN-major
     (void)scratch;
     BGemmArgs o{};
     o.A = P_out; o.B = V; o.C = O; o.M = n; o.N = D; o.K = n; o.lda = n; o.ldb = lq; o.ldc = lo; o.b_mn = 1;
     o.sAb = nn * H; o.sAh = nn; o.sBb = sb; o.sBh = sh; o.sCb = sbo; o.sCh = sh; o.H = H; o.alpha = 1.0f;
     o.drop_mode = 1; o.drop = make_drop(dropout_p, seed, offset);
-    if ((rc = launch_bgemm(o, Z, passes, st, "attn_tc_pv"))) return rc;
+    if ((rc = launch_bgemm(o, Z, st, "attn_tc_pv"))) return rc;
     return check_launch("attention_tc_fwd");
 }
 
@@ -462,6 +451,7 @@ int ptrb200_attention_tc_bwd_ld(const float* Q, const float* K, const float* V, 
                                 int B, int n, int H, int D, int ld_qkv, int ld_o, float dropout_p, uint64_t seed,
                                 uint64_t offset, int passes, ptrb200_stream_t stream) {
     if (!Q || !K || !V || !P || !dO || !dQ || !dK || !dV || !scratch || B <= 0 || n <= 0 || H <= 0 || D <= 0) { set_error("attention_tc_bwd: bad arguments"); return PTRB200_ERR_INVALID; }
+    if (passes != 3) { set_error("attention_tc_bwd: passes must be 3 (3xTF32), got %d", passes); return PTRB200_ERR_UNSUPPORTED; }
     cudaStream_t st = (cudaStream_t)stream;
     const int Z = B * H, HD = H * D;
     const int lq = ld_qkv > 0 ? ld_qkv : HD, lo = ld_o > 0 ? ld_o : HD;
@@ -475,25 +465,25 @@ int ptrb200_attention_tc_bwd_ld(const float* Q, const float* K, const float* V, 
     BGemmArgs a{};
     a.A = dO; a.B = V; a.C = dS; a.M = n; a.N = n; a.K = D; a.lda = lo; a.ldb = lq; a.ldc = n;
     a.sAb = sbo; a.sAh = sh; a.sBb = sb; a.sBh = sh; a.sCb = nn * H; a.sCh = nn; a.H = H; a.alpha = 1.0f;
-    if ((rc = launch_bgemm(a, Z, passes, st, "attn_tc_dp"))) return rc;
+    if ((rc = launch_bgemm(a, Z, st, "attn_tc_dp"))) return rc;
     const size_t rows = (size_t)Z * n;
     PTRB200_LAUNCH(softmax_bwd_rows_kernel, (unsigned)((rows + 7) / 8), 256, 0, st, P, dS, rows, n, inv_scale, drop);
     // dQ = dS K : K is the [K = key, N = d] factor (MN-major B)
     BGemmArgs q{};
     q.A = dS; q.B = K; q.C = dQ; q.M = n; q.N = D; q.K = n; q.lda = n; q.ldb = lq; q.ldc = lq; q.b_mn = 1;
     q.sAb = nn * H; q.sAh = nn; q.sBb = sb; q.sBh = sh; q.sCb = sb; q.sCh = sh; q.H = H; q.alpha = 1.0f;
-    if ((rc = launch_bgemm(q, Z, passes, st, "attn_tc_dq"))) return rc;
+    if ((rc = launch_bgemm(q, Z, st, "attn_tc_dq"))) return rc;
     // dK = dS^T Q : dS itself is the [K = query, M = key] factor (MN-major A), Q the [K = query, N = d] factor (MN-major B)
     BGemmArgs k{};
     k.A = dS; k.B = Q; k.C = dK; k.M = n; k.N = D; k.K = n; k.lda = n; k.ldb = lq; k.ldc = lq; k.a_mn = 1; k.b_mn = 1;
     k.sAb = nn * H; k.sAh = nn; k.sBb = sb; k.sBh = sh; k.sCb = sb; k.sCh = sh; k.H = H; k.alpha = 1.0f;
-    if ((rc = launch_bgemm(k, Z, passes, st, "attn_tc_dk"))) return rc;
+    if ((rc = launch_bgemm(k, Z, st, "attn_tc_dk"))) return rc;
     // dV = dropout(P)^T dO : same shapes, the dropout mask regenerated through the transposed view
     BGemmArgs v{};
     v.A = P; v.B = dO; v.C = dV; v.M = n; v.N = D; v.K = n; v.lda = n; v.ldb = lo; v.ldc = lq; v.a_mn = 1; v.b_mn = 1;
     v.sAb = nn * H; v.sAh = nn; v.sBb = sbo; v.sBh = sh; v.sCb = sb; v.sCh = sh; v.H = H; v.alpha = 1.0f;
     v.drop_mode = 2; v.drop = drop;
-    if ((rc = launch_bgemm(v, Z, passes, st, "attn_tc_dv"))) return rc;
+    if ((rc = launch_bgemm(v, Z, st, "attn_tc_dv"))) return rc;
     return check_launch("attention_tc_bwd");
 }
 

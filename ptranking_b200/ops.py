@@ -10,7 +10,6 @@ import contextlib
 import ctypes as C
 import functools
 import math
-import os
 from typing import Optional, Sequence
 
 import torch
@@ -1046,38 +1045,6 @@ def unpad_lists(padded: torch.Tensor, offsets: torch.Tensor, total: int) -> torc
     return _UnpadLists.apply(padded, _offsets_i32(offsets, padded.device), int(total))
 
 
-class _Attention(torch.autograd.Function):
-    @staticmethod
-    @_on_tensor_device
-    def forward(ctx, Q, K, V, n_heads, dropout_p, seed, offset):
-        lib = _lib.load()
-        Q, K, V = _dev_f32(Q, "Q"), _dev_f32(K, "K"), _dev_f32(V, "V")
-        B, n, F = Q.shape
-        D = F // n_heads
-        O = torch.empty_like(Q)
-        lse = torch.empty((B, n_heads, n), dtype=torch.float32, device=Q.device)
-        _lib.check(lib.ptrb200_attention_fwd(Q.data_ptr(), K.data_ptr(), V.data_ptr(), O.data_ptr(), lse.data_ptr(),
-                                             B, n, n_heads, D, float(dropout_p), seed, offset, _stream_ptr()), "attention_fwd")
-        ctx.save_for_backward(Q, K, V, O, lse)
-        ctx.cfg = (n_heads, float(dropout_p), seed, offset)
-        return O
-
-    @staticmethod
-    @_on_tensor_device
-    def backward(ctx, dO):
-        lib = _lib.load()
-        Q, K, V, O, lse = ctx.saved_tensors
-        H, p, seed, offset = ctx.cfg
-        B, n, F = Q.shape
-        dO = _dev_f32(dO, "dO")
-        dQ, dK, dV = torch.empty_like(Q), torch.empty_like(K), torch.empty_like(V)
-        scratch = torch.empty(B * H * n, dtype=torch.float32, device=Q.device)
-        _lib.check(lib.ptrb200_attention_bwd(Q.data_ptr(), K.data_ptr(), V.data_ptr(), O.data_ptr(), dO.data_ptr(),
-                                             lse.data_ptr(), dQ.data_ptr(), dK.data_ptr(), dV.data_ptr(), scratch.data_ptr(),
-                                             B, n, H, F // H, p, seed, offset, _stream_ptr()), "attention_bwd")
-        return dQ, dK, dV, None, None, None, None
-
-
 def _key_lens_ptr(B: int, device):
     """Device pointer of the active key-length vector (None outside :func:`key_lens_context`)."""
     if _key_lens is None:
@@ -1085,63 +1052,6 @@ def _key_lens_ptr(B: int, device):
     if _key_lens.numel() != B or _key_lens.device != device or _key_lens.dtype != torch.int32:
         raise ValueError("key_lens_context: expected an int32 vector with one entry per query on the tensors' device")
     return _key_lens.data_ptr()
-
-
-class _AttentionTC(torch.autograd.Function):
-    """Tensor-core attention: batched wgmma GEMMs around a materialised [B*H,n,n] probability tensor."""
-
-    @staticmethod
-    @_on_tensor_device
-    def forward(ctx, Q, K, V, n_heads, dropout_p, seed, offset, passes):
-        lib = _lib.load()
-        Q, K, V = _dev_f32(Q, "Q"), _dev_f32(K, "K"), _dev_f32(V, "V")
-        B, n, F = Q.shape
-        D = F // n_heads
-        O = torch.empty_like(Q)
-        P = torch.empty((B * n_heads, n, n), dtype=torch.float32, device=Q.device)
-        scratch = torch.empty(lib.ptrb200_attention_tc_workspace_floats(B, n, n_heads, D, 0), dtype=torch.float32, device=Q.device)
-        _lib.check(lib.ptrb200_attention_tc_fwd_ld(Q.data_ptr(), K.data_ptr(), V.data_ptr(), O.data_ptr(), P.data_ptr(),
-                                                   scratch.data_ptr(), B, n, n_heads, D, 0, 0, _key_lens_ptr(B, Q.device),
-                                                   float(dropout_p), seed, offset, passes, _stream_ptr()), "attention_tc_fwd")
-        ctx.save_for_backward(Q, K, V, P)
-        ctx.cfg = (n_heads, float(dropout_p), seed, offset, passes)
-        return O
-
-    @staticmethod
-    @_on_tensor_device
-    def backward(ctx, dO):
-        lib = _lib.load()
-        Q, K, V, P = ctx.saved_tensors
-        H, p, seed, offset, passes = ctx.cfg
-        B, n, F = Q.shape
-        dO = _dev_f32(dO, "dO")
-        dQ, dK, dV = torch.empty_like(Q), torch.empty_like(K), torch.empty_like(V)
-        scratch = torch.empty(lib.ptrb200_attention_tc_workspace_floats(B, n, H, F // H, 1), dtype=torch.float32, device=Q.device)
-        _lib.check(lib.ptrb200_attention_tc_bwd(Q.data_ptr(), K.data_ptr(), V.data_ptr(), P.data_ptr(), dO.data_ptr(),
-                                                dQ.data_ptr(), dK.data_ptr(), dV.data_ptr(), scratch.data_ptr(),
-                                                B, n, H, F // H, p, seed, offset, passes, _stream_ptr()), "attention_tc_bwd")
-        return dQ, dK, dV, None, None, None, None, None
-
-
-def attention(Q, K, V, n_heads: int, dropout_p: float = 0.0, seed: Optional[int] = None, offset: Optional[int] = None,
-              impl: Optional[str] = None):
-    """softmax(Q K^T / sqrt(d)) [dropout] V per head; Q,K,V: [B,n,H*d].
-
-    impl: "tc" (wgmma 3xTF32 GEMMs, default), "tc_tf32" (single-pass TF32), "simt" (flash-style fp32 FMA kernels);
-    None reads PTRANKING_B200_ATTN.  All three draw the same dropout stream."""
-    if seed is None:
-        seed = torch.initial_seed() & (2 ** 64 - 1)
-    if offset is None:
-        offset = next_dropout_offset()
-    if impl is None:
-        impl = os.environ.get("PTRANKING_B200_ATTN", "tc")
-    if impl == "simt":
-        if _key_lens is not None:
-            raise NotImplementedError("padded ragged batches need a tensor-core attention impl (PTRANKING_B200_ATTN=tc)")
-        return _Attention.apply(Q, K, V, int(n_heads), float(dropout_p), int(seed), int(offset))
-    if impl not in ("tc", "tc_tf32"):
-        raise ValueError(f"unknown attention impl {impl!r}")
-    return _AttentionTC.apply(Q, K, V, int(n_heads), float(dropout_p), int(seed), int(offset), 3 if impl == "tc" else 1)
 
 
 class _AdjacentRows(torch.autograd.Function):
@@ -1172,12 +1082,13 @@ def adjacent_rows(*ts: torch.Tensor) -> torch.Tensor:
 
 
 class _AttentionTCPacked(torch.autograd.Function):
-    """_AttentionTC over Q|K|V side by side in one [B,n,3*F] tensor (the output of one F -> 3F projection): the kernels
-    read the three column blocks in place through their row pitch and the backward pass fills one [B,n,3*F] gradient."""
+    """Tensor-core attention (3xTF32 wgmma GEMMs around a materialised [B*H,n,n] probability tensor) over Q|K|V side by
+    side in one [B,n,3*F] tensor (the output of one F -> 3F projection): the kernels read the three column blocks in place
+    through their row pitch and the backward pass fills one [B,n,3*F] gradient."""
 
     @staticmethod
     @_on_tensor_device
-    def forward(ctx, qkv, n_heads, dropout_p, seed, offset, passes):
+    def forward(ctx, qkv, n_heads, dropout_p, seed, offset):
         lib = _lib.load()
         qkv = _dev_f32(qkv, "qkv")
         B, n, F3 = qkv.shape
@@ -1189,9 +1100,9 @@ class _AttentionTCPacked(torch.autograd.Function):
         q = qkv.data_ptr()
         _lib.check(lib.ptrb200_attention_tc_fwd_ld(q, q + 4 * F, q + 8 * F, O.data_ptr(), P.data_ptr(), scratch.data_ptr(),
                                                    B, n, n_heads, D, F3, 0, _key_lens_ptr(B, qkv.device), float(dropout_p), seed, offset,
-                                                   passes, _stream_ptr()), "attention_tc_fwd")
+                                                   3, _stream_ptr()), "attention_tc_fwd")
         ctx.save_for_backward(qkv, P)
-        ctx.cfg = (n_heads, float(dropout_p), seed, offset, passes)
+        ctx.cfg = (n_heads, float(dropout_p), seed, offset)
         return O
 
     @staticmethod
@@ -1199,7 +1110,7 @@ class _AttentionTCPacked(torch.autograd.Function):
     def backward(ctx, dO):
         lib = _lib.load()
         qkv, P = ctx.saved_tensors
-        H, p, seed, offset, passes = ctx.cfg
+        H, p, seed, offset = ctx.cfg
         B, n, F3 = qkv.shape
         F = F3 // 3
         dO = _dev_f32(dO, "dO")
@@ -1208,28 +1119,20 @@ class _AttentionTCPacked(torch.autograd.Function):
         q, g = qkv.data_ptr(), dqkv.data_ptr()
         _lib.check(lib.ptrb200_attention_tc_bwd_ld(q, q + 4 * F, q + 8 * F, P.data_ptr(), dO.data_ptr(),
                                                    g, g + 4 * F, g + 8 * F, scratch.data_ptr(),
-                                                   B, n, H, F // H, F3, 0, p, seed, offset, passes, _stream_ptr()), "attention_tc_bwd")
-        return dqkv, None, None, None, None, None
+                                                   B, n, H, F // H, F3, 0, p, seed, offset, 3, _stream_ptr()), "attention_tc_bwd")
+        return dqkv, None, None, None, None
 
 
-def attention_impl() -> str:
-    return os.environ.get("PTRANKING_B200_ATTN", "tc")
-
-
-def attention_packed(qkv, n_heads: int, dropout_p: float = 0.0, seed: Optional[int] = None, offset: Optional[int] = None,
-                     impl: Optional[str] = None):
-    """:func:`attention` for Q|K|V stored side by side in the last dimension of one tensor (tensor-core paths only)."""
+def attention_packed(qkv, n_heads: int, dropout_p: float = 0.0, seed: Optional[int] = None, offset: Optional[int] = None):
+    """softmax(Q K^T / sqrt(d)) [dropout] V per head, with Q|K|V side by side in the last dimension of one [B,n,3*H*d]
+    tensor; returns [B,n,H*d].  Inside :func:`key_lens_context`, query b attends to its first lens[b] keys only."""
     if seed is None:
         seed = torch.initial_seed() & (2 ** 64 - 1)
     if offset is None:
         offset = next_dropout_offset()
-    if impl is None:
-        impl = attention_impl()
-    if impl not in ("tc", "tc_tf32"):
-        raise ValueError(f"attention_packed needs a tensor-core impl, got {impl!r}")
     if qkv.shape[-1] % (3 * n_heads) != 0:
         raise ValueError("last dimension must be 3 * n_heads * head_dim")
-    return _AttentionTCPacked.apply(qkv, int(n_heads), float(dropout_p), int(seed), int(offset), 3 if impl == "tc" else 1)
+    return _AttentionTCPacked.apply(qkv, int(n_heads), float(dropout_p), int(seed), int(offset))
 
 
 class _LayerNormRef(torch.autograd.Function):

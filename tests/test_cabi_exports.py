@@ -41,6 +41,25 @@ def test_ctypes_prototypes_match_header(lib_path):
     assert isinstance(lib.ptrb200_launch_count(), int)
 
 
+def test_attention_tc_entry_points_reject_passes_other_than_3(lib_path):
+    """The attention calls keep their `passes` argument for ABI stability; only 3 (3xTF32) is implemented, and any other
+    value is refused while the arguments are checked, before anything reaches the device."""
+    from ptranking_b200 import _lib
+    lib = _lib.load()
+    buf = (ctypes.c_float * 16)()
+    p = ctypes.addressof(buf)          # never dereferenced: the call returns at the argument check
+    B, n, H, D = 1, 4, 1, 4
+    calls = {
+        "attention_tc_fwd": lambda: lib.ptrb200_attention_tc_fwd(*[p] * 6, B, n, H, D, 0.0, 0, 0, 1, None),
+        "attention_tc_bwd": lambda: lib.ptrb200_attention_tc_bwd(*[p] * 9, B, n, H, D, 0.0, 0, 0, 1, None),
+        "attention_tc_fwd_ld": lambda: lib.ptrb200_attention_tc_fwd_ld(*[p] * 6, B, n, H, D, 0, 0, None, 0.0, 0, 0, 1, None),
+        "attention_tc_bwd_ld": lambda: lib.ptrb200_attention_tc_bwd_ld(*[p] * 9, B, n, H, D, 0, 0, 0.0, 0, 0, 1, None),
+    }
+    for name, call in calls.items():
+        with pytest.raises(_lib.B200LibraryError, match="passes must be 3"):
+            _lib.check(call(), name)
+
+
 def test_no_cpu_fallback():
     import torch
     import ptranking_b200

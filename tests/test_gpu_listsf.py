@@ -11,43 +11,62 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 
 
-@pytest.mark.parametrize("impl", ["simt", "tc"])
-@pytest.mark.parametrize("shape", [(2, 24, 2, 10), (3, 200, 2, 68), (1, 512, 2, 68), (2, 37, 4, 17), (1, 1, 2, 23), (2, 130, 1, 46)])
-def test_attention_matches_float64(shape, impl):
+def _attention(Q, K, V, H, p, seed=None, offset=None):
+    """The attention core over separate Q, K, V: the packed entry point on their concatenation (autograd splits the
+    [B,n,3F] gradient back into dQ, dK, dV).  F % 4 == 0 exactly when 3F % 4 == 0 and the K and V blocks start 16-byte
+    aligned, so each contraction takes the same kernel as it would with Q, K, V in three tensors."""
     from ptranking_b200 import ops
+    return ops.attention_packed(torch.cat((Q, K, V), -1), H, p, seed=seed, offset=offset)
+
+
+def _attention_float64(Q, K, V, H, dO, mask=None):
+    """float64 reference of list_ranker.py:226-248 with the dropout mask (kept elements already scaled) as a tensor:
+    returns O and dQ, dK, dV for the incoming gradient dO."""
+    B, n, F = Q.shape
+    D = F // H
+    q, k, v = (t.double().requires_grad_(True) for t in (Q, K, V))
+    split = lambda t: t.view(B, n, H, D).permute(0, 2, 1, 3)
+    att = torch.softmax(split(q) @ split(k).transpose(-1, -2) / np.sqrt(D), dim=-1)
+    if mask is not None:
+        att = att * mask.double().view(B, H, n, n)
+    o_ref = (att @ split(v)).permute(0, 2, 1, 3).reshape(B, n, H * D)
+    (o_ref * dO.double()).sum().backward()
+    return o_ref.detach(), q.grad, k.grad, v.grad
+
+
+@pytest.mark.parametrize("shape", [(2, 24, 2, 10), (3, 200, 2, 68), (1, 512, 2, 68), (2, 37, 4, 17), (1, 1, 2, 23), (2, 130, 1, 46)])
+def test_attention_matches_float64(shape):
     B, n, H, D = shape
     g = torch.Generator().manual_seed(B * 1000 + n)
     Q, K, V = (torch.randn(B, n, H * D, generator=g) for _ in range(3))
     dO = torch.randn(B, n, H * D, generator=g)
-    # float64 reference of list_ranker.py:226-248
-    q, k, v = (t.double().requires_grad_(True) for t in (Q, K, V))
-    split = lambda t: t.view(B, n, H, D).permute(0, 2, 1, 3)
-    att = torch.softmax(split(q) @ split(k).transpose(-1, -2) / np.sqrt(D), dim=-1)
-    o_ref = (att @ split(v)).permute(0, 2, 1, 3).reshape(B, n, H * D)
-    (o_ref * dO.double()).sum().backward()
+    refs = _attention_float64(Q, K, V, H, dO)
     Qc, Kc, Vc = (t.to(DEV).requires_grad_(True) for t in (Q, K, V))
-    o = ops.attention(Qc, Kc, Vc, H, 0.0, impl=impl)
+    o = _attention(Qc, Kc, Vc, H, 0.0)
     (o * dO.to(DEV)).sum().backward()
-    # fp32 FMA path vs the 3xTF32 tensor-core path (split accumulators keep it at fp32 grade; north-star bound: 1e-5)
-    tol_o, tol_g = (2e-6, 5e-6) if impl == "simt" else (3e-6, 5e-6)
-    assert rel_err(o.detach().cpu().numpy(), o_ref.detach().numpy()) <= tol_o
-    for name, a, b in (("dQ", Qc.grad, q.grad), ("dK", Kc.grad, k.grad), ("dV", Vc.grad, v.grad)):
-        assert rel_err(a.cpu().numpy(), b.numpy()) <= tol_g, name
+    # 3xTF32 tensor-core path: split accumulators keep it at fp32 grade (north-star bound: 1e-5)
+    for name, a, b, tol in zip(("O", "dQ", "dK", "dV"), (o.detach(), Qc.grad, Kc.grad, Vc.grad), refs, (3e-6, 5e-6, 5e-6, 5e-6)):
+        assert rel_err(a.cpu().numpy(), b.numpy()) <= tol, name
 
 
-def test_attention_tc_and_simt_share_the_dropout_stream():
+def test_attention_dropout_matches_float64():
+    """Dropout in the forward contraction, the softmax backward and the transposed dV contraction against float64 autograd
+    on softmax(QK^T/sqrt(d)) * M with the mask M drawn by the elementwise dropout kernel over ones [B*H, n, n]: that kernel
+    keys element i by its flat index, which is the attention's element id (z*n + row)*n + col.  (2, 152, 2, 68) takes the
+    alignment-specialised GEMM kernel; n = 150 and D = 46 take the general one."""
     from ptranking_b200 import ops
-    B, n, H, D = 2, 150, 2, 68
-    torch.manual_seed(3)
-    outs = {}
-    Q0, K0, V0, G = (torch.randn(B, n, H * D, device=DEV) for _ in range(4))
-    for impl in ("simt", "tc"):
-        Q, K, V = (t.clone().requires_grad_(True) for t in (Q0, K0, V0))
-        o = ops.attention(Q, K, V, H, 0.25, seed=11, offset=4, impl=impl)
-        (o * G).sum().backward()
-        outs[impl] = [t.detach().cpu().numpy() for t in (o, Q.grad, K.grad, V.grad)]
-    for a, b in zip(outs["simt"], outs["tc"]):
-        assert rel_err(b, a) <= 1e-5
+    p, seed, offset = 0.25, 11, 4
+    for B, n, H, D in ((2, 152, 2, 68), (2, 150, 2, 68), (2, 130, 1, 46)):
+        g = torch.Generator().manual_seed(B * 1000 + n + D)
+        Q, K, V, dO = (torch.randn(B, n, H * D, generator=g) for _ in range(4))
+        mask = ops._ew(ops.EW_DROPOUT, torch.ones(B * H, n, n, device=DEV), None, p, seed, offset).cpu()
+        assert 0.2 < float((mask == 0).double().mean()) < 0.3
+        refs = _attention_float64(Q, K, V, H, dO, mask)
+        Qc, Kc, Vc = (t.to(DEV).requires_grad_(True) for t in (Q, K, V))
+        o = _attention(Qc, Kc, Vc, H, p, seed=seed, offset=offset)
+        (o * dO.to(DEV)).sum().backward()
+        for name, a, b, tol in zip(("O", "dQ", "dK", "dV"), (o.detach(), Qc.grad, Kc.grad, Vc.grad), refs, (3e-6, 5e-6, 5e-6, 5e-6)):
+            assert rel_err(a.cpu().numpy(), b.numpy()) <= tol, ((B, n, H, D), name)
 
 
 @pytest.mark.parametrize("shape", [(2, 152, 2, 68), (1, 512, 2, 68), (3, 24, 2, 12), (2, 260, 1, 136), (2, 640, 2, 68), (2, 200, 4, 32)])
@@ -55,7 +74,6 @@ def test_attention_tc_and_simt_share_the_dropout_stream():
 def test_attention_tc_aligned_kernel_equals_general_kernel(shape, p, monkeypatch):
     """The alignment-specialised batched-GEMM kernel stages the same operand images and issues the same MMAs as the
     general one (which remains the path of shapes that are not multiples of four): identical bits, dropout included."""
-    from ptranking_b200 import ops
     B, n, H, D = shape
     torch.manual_seed(n)
     Q0, K0, V0, G = (torch.randn(B, n, H * D, device=DEV) for _ in range(4))
@@ -63,24 +81,21 @@ def test_attention_tc_aligned_kernel_equals_general_kernel(shape, p, monkeypatch
     for general in ("0", "1"):
         monkeypatch.setenv("PTRB200_BGEMM_GENERAL", general)
         Q, K, V = (t.clone().requires_grad_(True) for t in (Q0, K0, V0))
-        o = ops.attention(Q, K, V, H, p, seed=21, offset=2, impl="tc")
+        o = _attention(Q, K, V, H, p, seed=21, offset=2)
         (o * G).sum().backward()
         outs.append([t.detach().clone() for t in (o, Q.grad, K.grad, V.grad)])
     for a, b in zip(*outs):
         assert torch.equal(a, b)
 
 
-@pytest.mark.parametrize("impl", ["simt", "tc"])
-def test_attention_dropout_consistent_between_forward_and_backward(impl, monkeypatch):
-    from ptranking_b200 import ops
-    monkeypatch.setenv("PTRANKING_B200_ATTN", impl)
+def test_attention_dropout_consistent_between_forward_and_backward():
     B, n, H, D = 2, 96, 2, 16
     torch.manual_seed(0)
     Q, K = torch.randn(B, n, H * D, device=DEV), torch.randn(B, n, H * D, device=DEV)
     V = torch.randn(B, n, H * D, device=DEV, requires_grad=True)
-    o1 = ops.attention(Q, K, V, H, 0.3, seed=5, offset=9)
-    o2 = ops.attention(Q, K, V, H, 0.3, seed=5, offset=9)
-    o3 = ops.attention(Q, K, V, H, 0.3, seed=5, offset=10)
+    o1 = _attention(Q, K, V, H, 0.3, seed=5, offset=9)
+    o2 = _attention(Q, K, V, H, 0.3, seed=5, offset=9)
+    o3 = _attention(Q, K, V, H, 0.3, seed=5, offset=10)
     assert torch.equal(o1, o2) and not torch.equal(o1, o3)
     # O is linear in V for a fixed mask: finite-difference-free check  dL/dV . V == L  for L = sum(O*G)
     G = torch.randn_like(o1)
@@ -88,8 +103,8 @@ def test_attention_dropout_consistent_between_forward_and_backward(impl, monkeyp
     lhs = float((V.grad * V).sum()), float((o1 * G).sum())
     assert abs(lhs[0] - lhs[1]) <= 1e-3 * max(abs(lhs[1]), 1.0)
     # expectation over masks ~ no-dropout output
-    o0 = ops.attention(Q, K, V, H, 0.0)
-    mean = torch.stack([ops.attention(Q, K, V, H, 0.3, seed=7, offset=100 + i) for i in range(64)]).mean(0)
+    o0 = _attention(Q, K, V, H, 0.0)
+    mean = torch.stack([_attention(Q, K, V, H, 0.3, seed=7, offset=100 + i) for i in range(64)]).mean(0)
     assert float((mean - o0).abs().mean()) < 0.15 * float(o0.abs().mean())
 
 
