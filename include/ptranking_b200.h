@@ -216,6 +216,37 @@ int ptrb200_daletor_fwd_bwd(const float* scores, const int32_t* offsets, const f
                             const int32_t* sub_counts, float* grad, float* loss_per_query, int B, int n, int m, float rt,
                             float alpha, int top_k, ptrb200_stream_t stream);
 
+/* DivProbRanker, ltr_diversification/score_and_sort/div_prob_ranker.py + base/div_mdn_ranker.py:276-326, with
+ * opt_ideal (the ideal order is the input order).  raw: the scorer's output, [rows, out_dim] row-major with out_dim = 2
+ * for K = 1 (mean, raw variance) and 3K otherwise (K mixture logits | K means | K raw variances); the variance transform
+ * is exp, or limit_delta * sigmoid when limit_delta > 0.  Rows are cut into queries by offsets (or dense [B,n]).
+ * loss: PTRB200_DIVPROB_ANDCG (SuperSoft aNDCG; top_k slices subtopic rows), _NERRIA (SuperSoft nERR-IA; top_k slices
+ * documents), _PAIRCLS, _LAMBDA_PAIRCLS (norm != 0 divides the swap weights by the ideal alpha-DCG).  top_k <= 0: all.
+ * loss_per_query[q] and grad_raw = d loss_per_query[q] / d raw[rows of q]; workspace: floats at the rele blocks'
+ * offsets (the size of `rele`), written by the aNDCG and LambdaPairCLS losses, may be NULL for the others.  The pair
+ * probabilities are recomputed where needed, never stored.  One CTA per query, sums in a fixed order: a query's
+ * results are bit-identical alone or in any batch.  beta (alpha of alpha-nDCG) is 0.5, as in the reference. */
+#define PTRB200_DIVPROB_ANDCG          0
+#define PTRB200_DIVPROB_NERRIA         1
+#define PTRB200_DIVPROB_PAIRCLS        2
+#define PTRB200_DIVPROB_LAMBDA_PAIRCLS 3
+int ptrb200_divprob_fwd_bwd(const float* raw, int out_dim, const int32_t* offsets, const float* rele,
+                            const int64_t* rele_offsets, const int32_t* sub_counts, float* workspace, float* grad_raw,
+                            float* loss_per_query, int B, int n, int m, int K, float limit_delta, int loss, int top_k,
+                            int norm, ptrb200_stream_t stream);
+
+/* div_mdn_ranker.py:301-326: key[row] = mu (PTRB200_DIVPROB_KEY_EXPRELE), 1 / E (RERAR: the reciprocal of the expected
+ * rank within the row's query) or mu - 0.1 v (RISKAWARE), from the same raw layout and head as above. */
+#define PTRB200_DIVPROB_KEY_EXPRELE   0
+#define PTRB200_DIVPROB_KEY_RERAR     1
+#define PTRB200_DIVPROB_KEY_RISKAWARE 2
+int ptrb200_divprob_sort_key(const float* raw, int out_dim, const int32_t* offsets, float* key, int B, int n, int K,
+                             float limit_delta, int sort_id, ptrb200_stream_t stream);
+
+/* The head alone (div_mdn_ranker.py:276-299): mu[r], var[r] of each of `rows` raw rows, layout and transform as above. */
+int ptrb200_divprob_head(const float* raw, int out_dim, long long rows, int K, float limit_delta, float* mu, float* var,
+                         ptrb200_stream_t stream);
+
 /* torch_alpha_ndcg_at_ks / torch_err_ia_at_ks / torch_nerr_ia_at_ks (metric/srd/diversity_metric.py:50-103, 190-290)
  * after the evaluator's score sort (base/ranker.py:265-475): out[B][3][nks] = alpha-nDCG, ERR-IA, nERR-IA of the
  * ranking by score (descending, ties by ascending index) against the input order as the ideal; cutoffs > n_q give 0.

@@ -4,7 +4,7 @@
     ptranking_b200.install()           # swap the loss classes into ptranking.ltr_adhoc.eval.ltr
     LTREvaluator(cuda=0).run(model_id='LambdaRank', ...)   # the unmodified reference driver
 
-    ptranking_b200.install_diversification()   # DALETOR into ptranking.ltr_diversification.eval.ltr_diversification
+    ptranking_b200.install_diversification()   # DALETOR and DivProbRanker into ptranking.ltr_diversification.eval.ltr_diversification
     DivLTREvaluator(cuda=0).run(model_id='DALETOR', sf_id='pointsf', ...)
 
 Importing the package never touches the GPU; the first kernel call loads
@@ -23,11 +23,12 @@ from .ltr_adhoc.listwise.softrank import SoftRank
 from .ltr_adhoc.listwise.wassrank import WassRank
 from .ltr_adhoc.listwise.mdprank import MDPRank
 from .ltr_diversification.score_and_sort.daletor import DALETOR
+from .ltr_diversification.score_and_sort.div_prob_ranker import DivProbRanker
 from .base.ranker import LABEL_TYPE
 
 MODELS = {c.__name__: c for c in (RankNet, LambdaRank, LambdaLoss, ListNet, ListMLE, ApproxNDCG,
                                   RankMSE, RankCosine, STListNet, SoftRank, WassRank, MDPRank)}
-DIV_MODELS = {c.__name__: c for c in (DALETOR,)}
+DIV_MODELS = {c.__name__: c for c in (DALETOR, DivProbRanker)}
 __version__ = "0.1.0"
 
 
@@ -55,11 +56,13 @@ def install(module=None):
 
 def install_diversification(module=None):
     """Register the diversification classes where the reference's diversification driver resolves model ids by name:
-    ``globals()[model_id]`` in ptranking/ltr_diversification/eval/ltr_diversification.py:385-389."""
+    ``globals()[model_id]`` in ptranking/ltr_diversification/eval/ltr_diversification.py:385-389.  Returns
+    {name: the value it replaced} for the names the module already had (the reference's driver has all of them)."""
     if module is None:
         import ptranking.ltr_diversification.eval.ltr_diversification as module  # the reference must be importable
     previous = {}
     for name, cls in DIV_MODELS.items():
-        previous[name] = getattr(module, name, None)
+        if hasattr(module, name):
+            previous[name] = getattr(module, name)
         setattr(module, name, cls)
     return previous

@@ -77,6 +77,9 @@ SIGNATURES = {
     "ptrb200_wassrank_fwd_bwd": (_I, [_fp, _fp, _fp, _fp, _fp, _I, _I, _I, _I, _F, _I, _F, _F, _F, _fp]),
     "ptrb200_mdprank_fwd_bwd": (_I, [_fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _I, _I, _I, _F, _F, _I, _U64, _U64, _fp]),
     "ptrb200_daletor_fwd_bwd": (_I, [_fp, _fp, _fp, _fp, _fp, _fp, _fp, _I, _I, _I, _F, _F, _I, _fp]),
+    "ptrb200_divprob_fwd_bwd": (_I, [_fp, _I, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _I, _I, _I, _I, _F, _I, _I, _I, _fp]),
+    "ptrb200_divprob_sort_key": (_I, [_fp, _I, _fp, _fp, _I, _I, _I, _F, _I, _fp]),
+    "ptrb200_divprob_head": (_I, [_fp, _I, _I64, _I, _F, _fp, _fp, _fp]),
     "ptrb200_srd_metrics_at_ks": (_I, [_fp, _fp, _fp, _fp, _fp, C.POINTER(C.c_int32), _I, _fp, _fp, _fp, _I, _I, _I, _F,
                                        _F, _fp]),
     "ptrb200_div_features": (_I, [_fp, _fp, _fp, _fp, _I, _I, _I, _fp]),

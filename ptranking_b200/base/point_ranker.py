@@ -21,7 +21,8 @@ class PointNeuralRanker(NeuralRanker):
         # the scorer is a single fused op whose backward overwrites every parameter gradient: let it write
         # straight into the flat gradient bucket (no per-tensor accumulate kernels, no zero fill)
         self.point_sf.write_through_grads = True
-        self.grad_bucket_overwritten = True
+        # (a zero-padded output layer, StackedFFNet._pad_out, hands its gradients to autograd instead: zero the bucket)
+        self.grad_bucket_overwritten = not self.point_sf._pad_out
 
     def config_point_neural_scoring_function(self):
         point_sf = self.ini_pointsf(**self.sf_para_dict[self.sf_para_dict['sf_id']])

@@ -44,11 +44,19 @@ class StackedFFNet(nn.Module):
     """Dropout -> Linear -> (BN|BN2) -> AF per hidden layer, Linear [-> norm -> TL_AF] tail."""
 
     def __init__(self, ff_dims, AF=None, TL_AF=None, apply_tl_af=False, dropout=0.1,
-                 BN=True, bn_type=None, bn_affine=False, device=None, math_mode=None, bn_per_query=False):
+                 BN=True, bn_type=None, bn_affine=False, device=None, math_mode=None, bn_per_query=False,
+                 pad_output=False):
         """``bn_per_query`` (bn_type 'BN' only): normalise each query over its own documents, as the reference's BN does
         when it scores one query per call (the diversification rankers).  The parameters and checkpoint keys stay
         LTRBatchNorm's; the kernels run BN2's per-query statistics with gamma/beta = bn.weight/bn.bias (constant 1 / 0
-        without affine) and no second affine."""
+        without affine) and no second affine.
+        ``pad_output``: the tensor-core kernels take output widths up to 4 or multiples of 4, and per-query statistics
+        over a ragged batch run on them only; any other width sends the whole net to the fp32 SIMT kernels, which refuse
+        ragged per-query batches.  With ``pad_output`` such an output layer (DivProbRanker's 3K mixture outputs) is
+        computed zero-padded to the next multiple of 4 -- zero weight rows and bias, and for a normalised output layer
+        scale 1 / shift 0 -- and the first ff_dims[-1] columns are returned.  The padded columns are constant 0 before
+        the norm, so they change neither the other columns' statistics nor their gradients; parameters and checkpoint
+        keys keep their own shapes."""
         super().__init__()
         # "3xtf32" (default): wgmma tensor cores with the fp32-equivalent 3-pass TF32 split;
         # "tf32": single pass; "simt": fp32 FMA kernels (also the fallback for widths the MMA tiles reject)
@@ -67,6 +75,7 @@ class StackedFFNet(nn.Module):
         # .to() replaces
         self._order = []
         for i in range(1, L):
+            self._last = len(self._order)       # where the output layer's tensors begin, after the loop
             lin = nn.Linear(ff_dims[i - 1], ff_dims[i])
             nn.init.xavier_normal_(lin.weight)
             self.add_module(f"ff_{i + 1}", lin)
@@ -89,11 +98,25 @@ class StackedFFNet(nn.Module):
                 self.add_module(f"bn_{i + 1}", holder)
         self.bn_per_query = bool(bn_per_query)
         norm = ("BN2" if bn_per_query else bn_type) if BN else None
-        self.spec = ops.FFNetSpec(ff_dims, AF if L > 2 else None, TL_AF if apply_tl_af else None,
-                                  norm, bn_affine and not bn_per_query, dropout, math_mode=math_mode)
+        out = ff_dims[-1]
+        self._pad_out = (-out) % 4 if pad_output and out > 4 else 0
+        self.spec = ops.FFNetSpec(list(ff_dims[:-1]) + [out + self._pad_out], AF if L > 2 else None,
+                                  TL_AF if apply_tl_af else None, norm, bn_affine and not bn_per_query, dropout,
+                                  math_mode=math_mode)
 
     def ordered_parameters(self):
-        return [getattr(getattr(self, e[0]), e[1]) if isinstance(e, tuple) else e for e in self._order]
+        ps = [getattr(getattr(self, e[0]), e[1]) if isinstance(e, tuple) else e for e in self._order]
+        if self._pad_out:
+            # the output layer: weight and bias with zero rows appended, then its norm's (scale, shift) pairs -- gamma
+            # and beta, and BN2's affine weight and bias -- with 1 / 0
+            k = self._last
+            w = ps[k]
+            ps[k] = torch.cat((w, w.new_zeros(self._pad_out, w.shape[1])))
+            for j in range(k + 1, len(ps)):
+                t = ps[j]
+                fill = t.new_ones(self._pad_out) if (j - k) % 2 == 0 else t.new_zeros(self._pad_out)
+                ps[j] = torch.cat((t, fill))
+        return ps
 
     def _grad_targets(self):
         """p.grad of every parameter, and a scratch sink for each constant -- or None while some gradient storage is
@@ -123,14 +146,17 @@ class StackedFFNet(nn.Module):
         # when every parameter already owns gradient storage (the ranker's flat bucket), the backward kernels write
         # into it directly instead of handing autograd 2 tensors per layer to accumulate
         targets = None
-        if torch.is_grad_enabled() and getattr(self, "write_through_grads", False):
+        if torch.is_grad_enabled() and getattr(self, "write_through_grads", False) and not self._pad_out:
             targets = self._grad_targets()
         if ragged_bn2:
             if X.dim() != 2:
                 raise ValueError("a ragged batch is [total_docs, F]")
-            return ops.ffnet_apply(X, self.spec, self.ordered_parameters(), training=self.training, grad_targets=targets,
-                                   offsets=offsets, max_len=max_len)
+            out = ops.ffnet_apply(X, self.spec, self.ordered_parameters(), training=self.training, grad_targets=targets,
+                                  offsets=offsets, max_len=max_len)
+            return out[:, :out.shape[1] - self._pad_out].contiguous() if self._pad_out else out
         out = ops.ffnet_apply(X, self.spec, self.ordered_parameters(), training=self.training, grad_targets=targets)
+        if self._pad_out:
+            out = out[..., :out.shape[-1] - self._pad_out].contiguous()
         return out.squeeze(0) if squeeze else out
 
 

@@ -253,18 +253,6 @@ __global__ void div_list_rows_kernel(const float* __restrict__ src, long long ld
     }
 }
 
-static int check_rele_args(const char* who, const void* rele, const void* rele_offsets, const void* sub_counts, int m) {
-    if (!rele || !rele_offsets || !sub_counts || m <= 0) {
-        set_error("%s: null subtopic relevance arguments or non-positive m=%d", who, m);
-        return PTRB200_ERR_INVALID;
-    }
-    if (m > PTRB200_MAX_SUBTOPICS) {
-        set_error("%s: %d subtopics exceed PTRB200_MAX_SUBTOPICS=%d", who, m, PTRB200_MAX_SUBTOPICS);
-        return PTRB200_ERR_UNSUPPORTED;
-    }
-    return PTRB200_OK;
-}
-
 }  // namespace ptrb200
 
 using namespace ptrb200;

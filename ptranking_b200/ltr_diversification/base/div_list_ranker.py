@@ -95,7 +95,7 @@ class DivListNeuralRanker:
         encoder = Encoder(layer=layer, num_layers=encoder_layers, encoder_type=encoder_type)
         uni_sf = StackedFFNet([2 * W, *ff_dims, out_dim], AF=AF, TL_AF=TL_AF, apply_tl_af=apply_tl_af, dropout=0.1,
                               BN=BN, bn_type=bn_type, bn_affine=bn_affine, device=self.device,
-                              bn_per_query=bool(BN) and bn_type == 'BN')
+                              bn_per_query=bool(BN) and bn_type == 'BN', pad_output=True)
         return {'encoder': encoder.to(self.device), 'uni_sf': uni_sf.to(self.device)}
 
     def list_parameters(self):

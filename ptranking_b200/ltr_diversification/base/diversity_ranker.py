@@ -128,7 +128,7 @@ class DiversityNeuralRanker(PointNeuralRanker, DivListNeuralRanker):
         ff_dims = [num_features] + [h_dim] * num_layers + [out_dim]
         return StackedFFNet(ff_dims, AF=AF, TL_AF=TL_AF, apply_tl_af=apply_tl_af, dropout=dropout, BN=BN,
                             bn_type=bn_type, bn_affine=bn_affine, device=self.device,
-                            bn_per_query=bool(BN) and bn_type == 'BN')
+                            bn_per_query=bool(BN) and bn_type == 'BN', pad_output=True)
 
     def div_forward(self, q_repr, doc_reprs):
         """div_point_ranker.py:14-24 / div_list_ranker.py:61-85: q_repr [1,F], doc_reprs [n,F] -> [1,n]."""
@@ -146,18 +146,29 @@ class DiversityNeuralRanker(PointNeuralRanker, DivListNeuralRanker):
         """[total, 3F] scorer input of a ragged batch -> flat scores [total] (per-query BN statistics)."""
         return self.point_sf(X, offsets=offsets, max_len=max_len).view(-1)
 
+    def split_list_order(self):
+        """Whether a split's scorer input is packed as [q, d, q*d] (True) or [q, q*d, d]: the list scorer reads the
+        former, the pointwise scorer of DiversityNeuralRanker the latter.  A subclass whose pointwise scorer reads the
+        list order overrides this."""
+        return 'listsf' == self.sf_id
+
+    def split_sort_keys(self, preds, sp):
+        """The sort keys of a packed split from its scorer output ``preds`` (flat, as div_forward_ragged / list_scores
+        return it), in the split's row order.  The scores themselves by default."""
+        return preds
+
     def _split(self, data):
         """The packed device copy of ``data``, built on first use and cached for the dataset object (weakly where the
         object allows it, so the device copies of a finished fold's splits go with their datasets)."""
         try:
             sp = self._weak_splits.get(data)
             if sp is None:
-                sp = self._weak_splits[data] = _Split(data, self.device, 'listsf' == self.sf_id)
+                sp = self._weak_splits[data] = _Split(data, self.device, self.split_list_order())
             return sp
         except TypeError:                           # e.g. a plain list of query tuples
             hit = self._splits.get(id(data))
             if hit is None or hit[0] is not data:
-                hit = self._splits[id(data)] = (data, _Split(data, self.device, 'listsf' == self.sf_id))
+                hit = self._splits[id(data)] = (data, _Split(data, self.device, self.split_list_order()))
             return hit[1]
 
     # ---- training ----------------------------------------------------------------------------------------------- #
@@ -222,6 +233,7 @@ class DiversityNeuralRanker(PointNeuralRanker, DivListNeuralRanker):
                 preds = self.list_scores(sp.X, sp.plan(0, len(sp), self))
             else:
                 preds = self.div_forward_ragged(sp.X, sp.offsets, sp.max_len)
+            preds = self.split_sort_keys(preds, sp)
         res = ops.srd_metrics_at_ks(preds, sp.rele, ks, max_label=1.0 if max_label is None else max_label,
                                     offsets=sp.offsets, max_len=sp.max_len, return_order=return_order)
         return (sp, *res)

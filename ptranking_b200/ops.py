@@ -586,6 +586,107 @@ def daletor_loss(scores: torch.Tensor, rele: SubtopicRele, **params):
     return _DaletorLoss.apply(scores, rele, params)
 
 
+DIVPROB_LOSSES = {"aNDCG": 0, "nERR-IA": 1, "PairCLS": 2, "LambdaPairCLS": 3}   # PTRB200_DIVPROB_*
+DIVPROB_SORT_IDS = {"ExpRele": 0, "RERAR": 1, "RiskAware": 2}                  # PTRB200_DIVPROB_KEY_*
+
+
+def _divprob_layout(raw: torch.Tensor, K: int, offsets, max_len):
+    """-> (raw fp32 contiguous, B, n, offsets pointer).  ``raw``: the scorer's output, [B,n,out_dim] dense or
+    [total_docs,out_dim] with ``offsets``/``max_len``; out_dim = 2 for K = 1, 3K otherwise."""
+    u = _dev_f32(raw, "raw")
+    D = 2 if K == 1 else 3 * K
+    if u.shape[-1] != D:
+        raise ValueError(f"raw output of width {u.shape[-1]} for K={K} (expected {D})")
+    if offsets is None and u.dim() != 3:
+        raise ValueError(f"expected [B,n,{D}] raw output, got {tuple(u.shape)} (pass offsets= and max_len= when ragged)")
+    B, n, _, op = _list_layout(u[..., 0], offsets, max_len)
+    return u, B, n, op
+
+
+@_on_tensor_device
+def divprob_loss_and_grad(raw: torch.Tensor, rele: SubtopicRele, opt_id: str = "SuperSoft", metric: str = "aNDCG",
+                          K: int = 1, limit_delta: Optional[float] = None, top_k: Optional[int] = None,
+                          norm: bool = True, offsets: Optional[torch.Tensor] = None, max_len: Optional[int] = None):
+    """DivProbRanker's loss (div_prob_ranker.py:295-359, opt_ideal) for every query of a batch in one launch, from the
+    scorer's raw output through the Gaussian head (div_mdn_ranker.py:276-299) -> (batch loss = sum of the per-query
+    losses, per-query losses [B], d loss / d raw).  ``opt_id`` 'SuperSoft' with ``metric`` 'aNDCG' (``top_k`` slices
+    subtopic rows) or 'nERR-IA' (``top_k`` slices documents), 'PairCLS', or 'LambdaPairCLS' (``norm``: swap weights over
+    the ideal alpha-DCG).  ``limit_delta`` None: variances exp(u); otherwise limit_delta * sigmoid(u)."""
+    lib = _lib.load()
+    loss_id = DIVPROB_LOSSES[metric if opt_id == "SuperSoft" else opt_id]
+    u, B, n, op = _divprob_layout(raw, int(K), offsets, max_len)
+    if rele.sub_counts.numel() != B:
+        raise ValueError(f"{rele.sub_counts.numel()} subtopic blocks for {B} queries")
+    rp, rop, scp = rele._ptrs(u.device)
+    grad = torch.empty_like(u)
+    loss_q = torch.empty(B, dtype=torch.float32, device=u.device)
+    ws = torch.empty_like(rele.rele) if loss_id in (0, 3) else None
+    _lib.check(lib.ptrb200_divprob_fwd_bwd(u.data_ptr(), u.shape[-1], op, rp, rop, scp, None if ws is None else ws.data_ptr(),
+                                           grad.data_ptr(), loss_q.data_ptr(), B, n, max(rele.max_sub, 1), int(K),
+                                           float(limit_delta or 0.0), loss_id, int(top_k) if top_k else 0, int(bool(norm)),
+                                           _stream_ptr()), "divprob loss kernel")
+    return sum_f32(loss_q), loss_q, grad
+
+
+class _DivProbLoss(torch.autograd.Function):
+    """batch loss = sum of per-query DivProbRanker losses; backward hands the fused d loss / d raw to the scorer."""
+
+    @staticmethod
+    @_on_tensor_device
+    def forward(ctx, raw, rele, params):
+        loss, loss_q, grad = divprob_loss_and_grad(raw.detach(), rele, **params)
+        ctx.save_for_backward(grad)
+        ctx.mark_non_differentiable(loss_q)
+        ctx.set_materialize_grads(False)
+        return loss, loss_q
+
+    @staticmethod
+    @_on_tensor_device
+    def backward(ctx, g_loss, _g_lq):
+        (grad,) = ctx.saved_tensors
+        if g_loss is None:
+            return None, None, None
+        return _ew(EW_MUL_SCALAR, grad, g_loss.reshape(1)), None, None
+
+
+def divprob_loss(raw: torch.Tensor, rele: SubtopicRele, **params):
+    """(0-dim batch loss differentiable w.r.t. ``raw``, per-query losses [B]); ``params`` as divprob_loss_and_grad."""
+    return _DivProbLoss.apply(raw, rele, params)
+
+
+@_on_tensor_device
+def divprob_sort_key(raw: torch.Tensor, sort_id: str = "ExpRele", K: int = 1, limit_delta: Optional[float] = None,
+                     offsets: Optional[torch.Tensor] = None, max_len: Optional[int] = None) -> torch.Tensor:
+    """DivMDNRanker.div_predict (div_mdn_ranker.py:301-326) from the raw output -> sort keys with the raw output's
+    leading shape ([B,n] or [total_docs]): mu ('ExpRele'), mu - 0.1 v ('RiskAware') or 1 / E, the reciprocal of the
+    expected rank within the query ('RERAR').  Forward only."""
+    lib = _lib.load()
+    u, B, n, op = _divprob_layout(raw, int(K), offsets, max_len)
+    key = torch.empty(u.shape[:-1], dtype=torch.float32, device=u.device)
+    if key.numel():
+        _lib.check(lib.ptrb200_divprob_sort_key(u.data_ptr(), u.shape[-1], op, key.data_ptr(), B, n, int(K),
+                                                float(limit_delta or 0.0), DIVPROB_SORT_IDS[sort_id], _stream_ptr()),
+                   "divprob sort key")
+    return key
+
+
+@_on_tensor_device
+def divprob_head(raw: torch.Tensor, K: int = 1, limit_delta: Optional[float] = None):
+    """The Gaussian head alone (div_mdn_ranker.py:276-299): raw [..., out_dim] -> (mu, var), each of shape raw[..., 0].
+    Forward only (training differentiates through :func:`divprob_loss`)."""
+    lib = _lib.load()
+    u = _dev_f32(raw, "raw")
+    D = 2 if int(K) == 1 else 3 * int(K)
+    if u.shape[-1] != D:
+        raise ValueError(f"raw output of width {u.shape[-1]} for K={K} (expected {D})")
+    mu = torch.empty(u.shape[:-1], dtype=torch.float32, device=u.device)
+    var = torch.empty_like(mu)
+    if mu.numel():
+        _lib.check(lib.ptrb200_divprob_head(u.data_ptr(), D, mu.numel(), int(K), float(limit_delta or 0.0), mu.data_ptr(),
+                                            var.data_ptr(), _stream_ptr()), "divprob head")
+    return mu, var
+
+
 @_on_tensor_device
 def srd_metrics_at_ks(scores: torch.Tensor, rele: SubtopicRele, ks: Sequence[int], max_label: float, alpha: float = 0.5,
                       offsets: Optional[torch.Tensor] = None, max_len: Optional[int] = None, return_order: bool = False):

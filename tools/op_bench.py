@@ -11,7 +11,8 @@ import bench
 import ptranking_b200
 from ptranking_b200 import ops, LABEL_TYPE
 
-tag = sys.argv[1] if len(sys.argv) > 1 else "r02"
+args = [a for a in sys.argv[1:] if not a.startswith("--")]
+tag = args[0] if args else "r02"
 dev = "cuda:0"
 rng = np.random.default_rng(137)
 rows = []
@@ -37,6 +38,45 @@ def labels(B, n):
 
 
 HBM = bench.measured_peaks()["hbm_gbs"]
+
+def divprob_rows():
+    """DivProbRanker's fused loss kernel against an ATen restatement of the reference's loss (tests/divprob_oracle.py's
+    fp32 port: head, [m, n, n] temporaries, autograd) on the same GPU: 64 queries of n documents, m = 8 subtopic rows,
+    K = 1 and limit_delta = 0.01 (the reference's defaults).  The kernel takes the 64 queries in one launch; the
+    restatement runs them one query at a time, as the reference's training loop does."""
+    from tests import divprob_oracle as dpo
+    out = []
+    B, m = 64, 8
+    for n in (50, 300, 1000):
+        raws = [torch.from_numpy(dpo.draw_raw(rng, n, 1, 0.01, True)).to(dev) for _ in range(B)]
+        mats = [torch.from_numpy((rng.random((m, n)) < 0.2).astype(np.float32)).to(dev) for _ in range(B)]
+        u = torch.stack(raws)
+        rele = ops.SubtopicRele.pack([R.cpu() for R in mats], dev)
+        for loss in dpo.LOSSES:
+            opt_id, metric = ("SuperSoft", loss) if loss in ("aNDCG", "nERR-IA") else (loss, None)
+            kw = dict(K=1, limit_delta=0.01, top_k=None, norm=True)
+            ms_k = timeit(lambda: ops.divprob_loss_and_grad(u, rele, opt_id=opt_id, metric=metric, **kw))
+
+            def aten():
+                for q in range(B):
+                    leaf = raws[q].unsqueeze(0).clone().requires_grad_(True)
+                    mus, vars = dpo.port_head(leaf, 1, 0.01)
+                    dpo.port_loss(mus, vars, mats[q], loss, None, True).backward()
+            ms_a = timeit(aten, iters=3, warm=1)
+            out.append((f"DivProbRanker {loss} K=1 limit 0.01: fused kernel", f"B={B} n={n} m={m}", ms_k, B / ms_k * 1e3,
+                        float('nan'), float('nan')))
+            out.append((f"DivProbRanker {loss}: ATen restatement, one query per call (x{ms_a / ms_k:.0f})",
+                        f"B={B} n={n} m={m}", ms_a, B / ms_a * 1e3, float('nan'), float('nan')))
+    return out
+
+
+if "--divprob" in sys.argv:
+    print(f"{torch.cuda.get_device_name()}")
+    print("| op | shape | ms | queries/s |\n|---|---|---|---|")
+    for name, shape, ms, qps, _, _ in divprob_rows():
+        print(f"| {name} | {shape} | {ms:.4f} | {qps:,.0f} |")
+    sys.exit(0)
+
 for name, params, shapes in [
     ("LambdaRank", dict(sigma=1.0), [(1024, 256), (256, 1024), (4096, 32)]),
     ("RankNet", dict(sigma=1.0), [(1024, 256)]),
@@ -81,6 +121,7 @@ for (B, n) in [(1024, 256), (64, 4096)]:
     rows.append(("DALETOR m=8 k=10", f"B={B} n={n}", ms, B / ms * 1e3, algo / ms / 1e6, algo / ms / 1e6 / HBM))
     ms = timeit(lambda: ops.srd_metrics_at_ks(s, rele, [1, 3, 5, 10, 20], max_label=1.0))
     rows.append(("alpha-nDCG+ERR-IA+nERR-IA @5 cutoffs m=8", f"B={B} n={n}", ms, B / ms * 1e3, algo / ms / 1e6, algo / ms / 1e6 / HBM))
+rows += divprob_rows()
 # ndcg / all metrics
 for (B, n) in [(1024, 256), (256, 1024)]:
     s = torch.randn(B, n, device=dev); y = labels(B, n)
