@@ -774,14 +774,42 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
                 live[h] = r < nrows;
                 orow[h] = g.Out + (size_t)(row0 + min(r, nrows - 1)) * N;
             }
+            if (MODE == RG_FWD) {
 #pragma unroll
-            for (int e = 0; e < NPc / 2; ++e) {
-                const int col = tc::acc_col(e);
-                if (col >= N) { acc[e] = 0.0f; continue; }
-                if (MODE == RG_FWD) acc[e] += __ldg(bias + col);
-                else if (g.drop.thr) {
-                    const int r = wg * 64 + tc::acc_row(e);
-                    acc[e] = dropout_keep(g.drop.key, (uint64_t)(row0 + r) * N + col, g.drop.thr) ? acc[e] * g.drop.scale : 0.0f;
+                for (int e = 0; e < NPc / 2; ++e) {
+                    const int col = tc::acc_col(e);
+                    if (col >= N) { acc[e] = 0.0f; continue; }
+                    acc[e] += __ldg(bias + col);
+                }
+            } else if (g.drop.thr && (N & 3) == 0) {
+                // Accumulators e..e+3 (e % 4 == 0) are columns col, col + 1 of rows r and r + 8; lanes l and l ^ 1 together
+                // hold the four columns of one quad of the dropout stream, whose mask is one 64-bit draw.  Each lane draws
+                // one of the two rows' quads (even lane: row r, odd lane: row r + 8) and passes its partner the 32 bits
+                // of that draw the partner's columns use: one draw per four elements instead of one per element.
+                const bool odd = lane & 1;
+#pragma unroll
+                for (int e = 0; e < NPc / 2; e += 4) {
+                    const int col = tc::acc_col(e);
+                    const uint64_t el = (uint64_t)(row0 + wg * 64 + tc::acc_row(e) + (odd ? 8 : 0)) * N + (col & ~3);
+                    const uint64_t d = dropout_draw4(g.drop.key, el >> 2);
+                    const uint32_t other = __shfl_xor_sync(0xffffffffu, odd ? (uint32_t)d : (uint32_t)(d >> 32), 1);
+                    const uint32_t ur = odd ? other : (uint32_t)d;               // row r: 16 bits per column
+                    const uint32_t ur8 = odd ? (uint32_t)(d >> 32) : other;      // row r + 8
+                    if (col >= N) { acc[e] = acc[e + 1] = acc[e + 2] = acc[e + 3] = 0.0f; continue; }   // (N % 4 == 0: col + 1 < N)
+                    acc[e] = (ur & 0xffffu) >= g.drop.thr ? acc[e] * g.drop.scale : 0.0f;
+                    acc[e + 1] = (ur >> 16) >= g.drop.thr ? acc[e + 1] * g.drop.scale : 0.0f;
+                    acc[e + 2] = (ur8 & 0xffffu) >= g.drop.thr ? acc[e + 2] * g.drop.scale : 0.0f;
+                    acc[e + 3] = (ur8 >> 16) >= g.drop.thr ? acc[e + 3] * g.drop.scale : 0.0f;
+                }
+            } else {
+#pragma unroll
+                for (int e = 0; e < NPc / 2; ++e) {
+                    const int col = tc::acc_col(e);
+                    if (col >= N) { acc[e] = 0.0f; continue; }
+                    if (g.drop.thr) {
+                        const int r = wg * 64 + tc::acc_row(e);
+                        acc[e] = dropout_keep(g.drop.key, (uint64_t)(row0 + r) * N + col, g.drop.thr) ? acc[e] * g.drop.scale : 0.0f;
+                    }
                 }
             }
             // a thread holds two adjacent columns of two rows per 8-column group: 8-byte stores when N is even
@@ -798,29 +826,32 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_gemm_ws_kernel(RowsGemmArg
 #pragma unroll
                 for (int j = 0; j < NPc / 16; ++j) {
                     const float* w = acc + 8 * j;
-                    // column sums over the warp's 16 rows: lanes with equal lane % 4 hold the same columns
-                    float s1[4], s2[4];
+                    // column sums over the warp's 16 rows: lanes with equal lane % 4 hold the same columns.
+                    // s[p] = sum, s[4 + p] = sum of squares of the lane's column p over its two rows
+                    float s[8];
 #pragma unroll
                     for (int p = 0; p < 4; ++p) {              // p = 2 * (e >> 2) + (e & 1): the four columns of this lane
                         const int e0 = (p >> 1) * 4 + (p & 1), e1 = e0 + 2;
                         const float v0 = live[0] ? w[e0] : 0.0f, v1 = live[1] ? w[e1] : 0.0f;
-                        s1[p] = v0 + v1; s2[p] = v0 * v0 + v1 * v1;
+                        s[p] = v0 + v1; s[4 + p] = v0 * v0 + v1 * v1;
                     }
+                    // reduce-scatter over the 8 lanes of equal lane % 4, partners lane ^ 4, ^ 8, ^ 16: each step adds the
+                    // same pairs a butterfly all-reduce adds (so the sums are the same bits) but keeps only half of the
+                    // values, 7 shuffles instead of 24.  Lane sl ends with the full sum of value 4 b2 + 2 b3 + b4 (bits of sl).
 #pragma unroll
-                    for (int p = 0; p < 4; ++p)
+                    for (int st = 0; st < 3; ++st) {
+                        const int h = 4 >> st, o = 4 << st;
+                        const bool up = sl & o;
 #pragma unroll
-                        for (int o = 4; o < 32; o <<= 1) {
-                            s1[p] += __shfl_xor_sync(0xffffffffu, s1[p], o);
-                            s2[p] += __shfl_xor_sync(0xffffffffu, s2[p], o);
-                        }
-                    if (sl < 4) {
-#pragma unroll
-                        for (int p = 0; p < 4; ++p) {
-                            const int col = j * 16 + (p >> 1) * 8 + 2 * sl + (p & 1);
-                            stat_sm[(sw * NP + col) * 2] = s1[p];
-                            stat_sm[(sw * NP + col) * 2 + 1] = s2[p];
+                        for (int i = 0; i < h; ++i) {
+                            float keep = s[i], send = s[i + h];
+                            if (up) { const float t = keep; keep = send; send = t; }
+                            s[i] = keep + __shfl_xor_sync(0xffffffffu, send, o);
                         }
                     }
+                    const int v = ((sl >> 2) & 1) * 4 + ((sl >> 3) & 1) * 2 + ((sl >> 4) & 1), p = v & 3;
+                    const int col = j * 16 + (p >> 1) * 8 + 2 * (sl & 3) + (p & 1);
+                    stat_sm[(sw * NP + col) * 2 + (v >> 2)] = s[0];
                 }
                 asm volatile("bar.sync 2, 256;" ::: "memory");               // the 8 warps' column sums are in smem
                 if (tid < N) {
