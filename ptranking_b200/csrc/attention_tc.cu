@@ -435,7 +435,7 @@ int ptrb200_attention_tc_fwd_ld(const float* Q, const float* K, const float* V, 
     BGemmArgs o{};
     o.A = P_out; o.B = V; o.C = O; o.M = n; o.N = D; o.K = n; o.lda = n; o.ldb = lq; o.ldc = lo; o.b_mn = 1;
     o.sAb = nn * H; o.sAh = nn; o.sBb = sb; o.sBh = sh; o.sCb = sbo; o.sCh = sh; o.H = H; o.alpha = 1.0f;
-    o.drop_mode = 1; o.drop = make_drop(dropout_p, seed, offset);
+    o.drop_mode = 1; o.drop = make_drop_call(dropout_p, seed, offset);
     if ((rc = launch_bgemm(o, Z, st, "attn_tc_pv"))) return rc;
     return check_launch("attention_tc_fwd");
 }
@@ -458,7 +458,7 @@ int ptrb200_attention_tc_bwd_ld(const float* Q, const float* K, const float* V, 
     if (lq < HD || lo < HD) { set_error("attention_tc_bwd: row pitch below H*D"); return PTRB200_ERR_INVALID; }
     const long long sb = (long long)n * lq, sbo = (long long)n * lo, sh = D, nn = (long long)n * n;
     float* dS = scratch;                    // [Z,n,n]
-    const DropCfg drop = make_drop(dropout_p, seed, offset);
+    const DropCfg drop = make_drop_call(dropout_p, seed, offset);
     const float inv_scale = 1.0f / sqrtf((float)D);
     int rc;
     // dA_d = dO V^T

@@ -162,8 +162,14 @@ __host__ __device__ __forceinline__ uint32_t dropout_bits(uint64_t seed, uint64_
 
 // ---- dropout masks: splitmix64 counter stream, 16 random bits per element ---------------------------
 // One 64-bit draw covers 4 consecutive elements (element e uses bits [16*(e&3), 16*(e&3)+16) of draw e>>2);
-// an element is KEPT when its 16-bit value >= thr = round(p * 65536).  The mask of an element depends only
-// on (key, element index), so forward, backward and every kernel variant regenerate identical masks.
+// an element is KEPT when its 16-bit value >= thr = round(p * 65536) and then scaled by 65536 / (65536 - thr).
+// The mask of an element depends only on (key, element index), so forward, backward and every kernel variant
+// regenerate identical masks.  Keys: dropout_key(seed, index) with
+//   index = o*64 + l   the input of Linear layer l of a stacked-FF call at offset o (make_drop), element
+//                      row * d_in(l) + col of the unpadded layer input;
+//   index = o*64 + 63  a call at offset o that draws a single mask: elementwise dropout, attention (make_drop_call).
+// Both kinds take o from the same counter (ops.next_dropout_offset); the FF net's layer slots stay below 63, so
+// no two calls share a stream.
 __host__ __device__ __forceinline__ uint64_t mix64(uint64_t x) {
     x ^= x >> 30; x *= 0xbf58476d1ce4e5b9ull;
     x ^= x >> 27; x *= 0x94d049bb133111ebull;
@@ -186,6 +192,10 @@ static inline DropCfg make_drop(float p, uint64_t seed, uint64_t offset) {
     d.scale = d.thr ? 65536.0f / (float)(65536u - d.thr) : 1.0f;
     d.key = dropout_key(seed, offset);
     return d;
+}
+static_assert(PTRB200_MAX_FF_LAYERS < 63, "the FF net's per-layer key slots must stay below the one-mask slot 63");
+static inline DropCfg make_drop_call(float p, uint64_t seed, uint64_t offset) {
+    return make_drop(p, seed, offset * 64 + 63);
 }
 
 }  // namespace ptrb200

@@ -812,23 +812,32 @@ __global__ void dgrad_rank1_kernel(const float* __restrict__ dz, const float* __
 }
 
 // dst[r, 0..kd) = src[r, 0..ks) (zero beyond ks when widening; truncated when narrowing): the zero-padding of the feature
-// matrix / first weight matrix to a multiple of 4 columns, and the way back for their gradients
-__global__ void copy_cols_kernel(const float* __restrict__ src, float* __restrict__ dst, size_t rows, int ks, int kd) {
+// matrix / first weight matrix to a multiple of 4 columns, and the way back for their gradients.
+// drop.thr != 0: layer 0's dropout mask is applied on the way, keyed by the element's index r * min(ks, kd) + k in the
+// unpadded matrix -- the index every other kernel variant uses -- so the padded features carry the same mask.
+static __device__ __forceinline__ float copy_drop(float v, const DropCfg& drop, size_t r, int k, int kl) {
+    return (!drop.thr || k >= kl || dropout_keep(drop.key, (uint64_t)r * kl + k, drop.thr)) ? v * drop.scale : 0.0f;
+}
+__global__ void copy_cols_kernel(const float* __restrict__ src, float* __restrict__ dst, size_t rows, int ks, int kd, DropCfg drop) {
     const size_t total = rows * (size_t)kd;
+    const int kl = ks < kd ? ks : kd;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
         const size_t r = i / kd;
         const int k = (int)(i - r * kd);
-        dst[i] = k < ks ? src[r * ks + k] : 0.0f;
+        const float v = k < ks ? src[r * ks + k] : 0.0f;
+        dst[i] = drop.thr ? copy_drop(v, drop, r, k, kl) : v;
     }
 }
 // the same from bf16 features (exact widening): the padded fp32 copy of a bf16 feature matrix (ks % 4 != 0), and with
 // kd == ks the fp32 copy the SIMT kernels read
-__global__ void copy_cols_bf16_kernel(const uint16_t* __restrict__ src, float* __restrict__ dst, size_t rows, int ks, int kd) {
+__global__ void copy_cols_bf16_kernel(const uint16_t* __restrict__ src, float* __restrict__ dst, size_t rows, int ks, int kd, DropCfg drop) {
     const size_t total = rows * (size_t)kd;
+    const int kl = ks < kd ? ks : kd;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
         const size_t r = i / kd;
         const int k = (int)(i - r * kd);
-        dst[i] = k < ks ? __uint_as_float((uint32_t)src[r * ks + k] << 16) : 0.0f;
+        const float v = k < ks ? __uint_as_float((uint32_t)src[r * ks + k] << 16) : 0.0f;
+        dst[i] = drop.thr ? copy_drop(v, drop, r, k, kl) : v;
     }
 }
 
@@ -1179,8 +1188,10 @@ static void set_norm_grads(DyTail& t, const ptrb200_ffnet* net, const ptrb200_ff
 // normalisation step: per-query bn2_ragged_* kernels on a materialised layer input instead of the epilogue statistics
 // partials and the normalisation folded into the next layer's prologue.
 // xb: X holds bf16 features, read natively by layer 0's forward and weight-gradient kernels.
-static int forward_tc(const ptrb200_ffnet* net, const Plan& p, const float* X, bool xb, const int32_t* offsets, float* out, char* ws,
-                      float drop, uint64_t seed, uint64_t offset, cudaStream_t st, bool fwd_only) {
+// x_masked: X already carries layer 0's dropout (the zero-padded copy of a feature matrix whose width is not a multiple
+// of 4), so layer 0 draws no mask of its own.
+static int forward_tc(const ptrb200_ffnet* net, const Plan& p, const float* X, bool xb, bool x_masked, const int32_t* offsets, float* out,
+                      char* ws, float drop, uint64_t seed, uint64_t offset, cudaStream_t st, bool fwd_only) {
     int rc;
     pack_weight_images(net, p, ws, fwd_only, st);
     for (int l = 0; l < p.L; ++l) {
@@ -1191,7 +1202,7 @@ static int forward_tc(const ptrb200_ffnet* net, const Plan& p, const float* X, b
         g.round_bf16 = p.bf16;
         set_prologue(net, p, l, ws, X, g.P, g.scale, g.shift, g.act);
         g.gr_prev = p.gr;
-        g.drop = make_drop(last ? 0.0f : drop, seed, offset * 64 + (uint64_t)l);
+        g.drop = make_drop((last || (l == 0 && x_masked)) ? 0.0f : drop, seed, offset * 64 + (uint64_t)l);
         g.bias = net->bias[l]; g.Out = Z;
         g.a_out = (l > 0 && !fwd_only) ? reinterpret_cast<float*>(ws + lp.ain_off) : nullptr;     // a by-product for the backward pass
         g.partials = (lp.has_norm && !p.ragged) ? reinterpret_cast<double*>(ws + p.partials_off) : nullptr;
@@ -1235,8 +1246,9 @@ static int forward_tc(const ptrb200_ffnet* net, const Plan& p, const float* X, b
     return check_launch("ffnet_forward(tc)");
 }
 
-static int backward_tc(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, const Plan& p, const float* X, bool xb, const int32_t* offsets,
-                       const float* dOut, float* dX, char* ws, float drop, uint64_t seed, uint64_t offset, cudaStream_t st) {
+static int backward_tc(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, const Plan& p, const float* X, bool xb, bool x_masked,
+                       const int32_t* offsets, const float* dOut, float* dX, char* ws, float drop, uint64_t seed, uint64_t offset,
+                       cudaStream_t st) {
     int rc;
     double* part = reinterpret_cast<double*>(ws + p.partials_off);
     float* S1 = reinterpret_cast<float*>(ws + p.s1_off);
@@ -1301,7 +1313,8 @@ static int backward_tc(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grad
             launch_colstat<STAT_COLSUM>(st, "colstat_colsum", dA, nullptr, nullptr, nr, part, G, p.S_stat, gr, lp.d_out, p.slice_rows);
             PTRB200_LAUNCH(dy_finalize_kernel, lp.d_out, FIN_THREADS, 0, st, (const double*)part, (float*)nullptr, (float*)nullptr, grads->bias[l], (float*)nullptr, G, lp.d_out, p.S_stat, DyTail{});
         }
-        const DropCfg layer_drop = make_drop(last ? 0.0f : drop, seed, offset * 64 + (uint64_t)l);
+        // (x_masked: layer 0's input already carries its mask, and the caller applies it to dX)
+        const DropCfg layer_drop = make_drop((last || (l == 0 && x_masked)) ? 0.0f : drop, seed, offset * 64 + (uint64_t)l);
         {   // dW = sum_rows dZ^T (x) layer input: dropout(X) rebuilt on the fly for layer 0, the operand the forward kernel built for deeper layers
             WgradArgs w{};
             w.round_bf16 = p.bf16;
@@ -1399,20 +1412,24 @@ int ptrb200_ffnet_forward_x(const ptrb200_ffnet* net, const void* Xv, int x_dtyp
     const float* X = static_cast<const float*>(Xv);       // bf16: reinterpreted by the kernels that read it (xb)
     bool xb = p.x_bf16;
     ptrb200_ffnet padded;
+    const DropCfg no_drop = make_drop(0.0f, 0, 0);
     if (p.pad_k) {          // zero-pad the features and the first weight matrix to a multiple of 4 columns (make_plan)
+        // layer 0's dropout is applied in the copy, keyed by the unpadded index row * dims[0] + k (a padded index would
+        // draw other masks than the SIMT path and the same features at their own width)
+        const DropCfg d0 = make_drop(p.L > 1 ? drop : 0.0f, seed, offset * 64);
         float* Xp = reinterpret_cast<float*>(ws + p.xpad_off);
         float* Wp = reinterpret_cast<float*>(ws + p.w0pad_off);
-        if (xb) PTRB200_LAUNCH(copy_cols_bf16_kernel, elementwise_blocks(p.rows * p.pad_k), 256, 0, st, static_cast<const uint16_t*>(Xv), Xp, p.rows, net->dims[0], p.pad_k);
-        else PTRB200_LAUNCH(copy_cols_kernel, elementwise_blocks(p.rows * p.pad_k), 256, 0, st, X, Xp, p.rows, net->dims[0], p.pad_k);
-        PTRB200_LAUNCH(copy_cols_kernel, elementwise_blocks((size_t)net->dims[1] * p.pad_k), 256, 0, st, net->weight[0], Wp, (size_t)net->dims[1], net->dims[0], p.pad_k);
+        if (xb) PTRB200_LAUNCH(copy_cols_bf16_kernel, elementwise_blocks(p.rows * p.pad_k), 256, 0, st, static_cast<const uint16_t*>(Xv), Xp, p.rows, net->dims[0], p.pad_k, d0);
+        else PTRB200_LAUNCH(copy_cols_kernel, elementwise_blocks(p.rows * p.pad_k), 256, 0, st, X, Xp, p.rows, net->dims[0], p.pad_k, d0);
+        PTRB200_LAUNCH(copy_cols_kernel, elementwise_blocks((size_t)net->dims[1] * p.pad_k), 256, 0, st, net->weight[0], Wp, (size_t)net->dims[1], net->dims[0], p.pad_k, no_drop);
         padded = *net; padded.dims[0] = p.pad_k; padded.weight[0] = Wp;
         net = &padded; X = Xp; xb = false;
     } else if (xb && !p.use_tc) {       // the SIMT kernels read fp32: widen once into the workspace (backward reads it too)
         float* Xw = reinterpret_cast<float*>(ws + p.xwide_off);
-        PTRB200_LAUNCH(copy_cols_bf16_kernel, elementwise_blocks(p.rows * net->dims[0]), 256, 0, st, static_cast<const uint16_t*>(Xv), Xw, p.rows, net->dims[0], net->dims[0]);
+        PTRB200_LAUNCH(copy_cols_bf16_kernel, elementwise_blocks(p.rows * net->dims[0]), 256, 0, st, static_cast<const uint16_t*>(Xv), Xw, p.rows, net->dims[0], net->dims[0], no_drop);
         X = Xw; xb = false;
     }
-    if (p.use_tc) return forward_tc(net, p, X, xb, offsets, out, ws, drop, seed, offset, st, (training & PTRB200_FFNET_FORWARD_ONLY) != 0);
+    if (p.use_tc) return forward_tc(net, p, X, xb, p.pad_k != 0, offsets, out, ws, drop, seed, offset, st, (training & PTRB200_FFNET_FORWARD_ONLY) != 0);
     const float* in = X;
     for (int l = 0; l < p.L; ++l) {
         const LayerPlan& lp = p.layer[l];
@@ -1479,14 +1496,16 @@ int ptrb200_ffnet_backward_x(const ptrb200_ffnet* net, const ptrb200_ffnet_grads
         pg.weight[0] = reinterpret_cast<float*>(ws + p.dw0pad_off);
         float* dXp = dX ? reinterpret_cast<float*>(ws + p.dxpad_off) : nullptr;
         const float* Xp = reinterpret_cast<const float*>(ws + p.xpad_off);
-        if ((rc = backward_tc(&padded, &pg, p, Xp, false, offsets, dOut, dXp, ws, drop, seed, offset, st))) return rc;
+        // Xp carries layer 0's dropout (forward call): layer 0 runs unmasked and its mask is applied to dX in the un-pad copy
+        if ((rc = backward_tc(&padded, &pg, p, Xp, false, true, offsets, dOut, dXp, ws, drop, seed, offset, st))) return rc;
         if (!grads->weight[0]) { set_error("ffnet_backward: layer 0 grad buffer NULL"); return PTRB200_ERR_INVALID; }
         PTRB200_LAUNCH(copy_cols_kernel, elementwise_blocks((size_t)net->dims[1] * net->dims[0]), 256, 0, st, (const float*)pg.weight[0], grads->weight[0],
-                       (size_t)net->dims[1], p.pad_k, net->dims[0]);
-        if (dX) PTRB200_LAUNCH(copy_cols_kernel, elementwise_blocks(p.rows * net->dims[0]), 256, 0, st, (const float*)dXp, dX, p.rows, p.pad_k, net->dims[0]);
+                       (size_t)net->dims[1], p.pad_k, net->dims[0], make_drop(0.0f, 0, 0));
+        if (dX) PTRB200_LAUNCH(copy_cols_kernel, elementwise_blocks(p.rows * net->dims[0]), 256, 0, st, (const float*)dXp, dX, p.rows, p.pad_k, net->dims[0],
+                               make_drop(p.L > 1 ? drop : 0.0f, seed, offset * 64));
         return check_launch("ffnet_backward(padded)");
     }
-    if (p.use_tc) return backward_tc(net, grads, p, X, xb, offsets, dOut, dX, ws, drop, seed, offset, st);
+    if (p.use_tc) return backward_tc(net, grads, p, X, xb, false, offsets, dOut, dX, ws, drop, seed, offset, st);
     double* part = reinterpret_cast<double*>(ws + p.partials_off);
     float* S1 = reinterpret_cast<float*>(ws + p.s1_off);
     float* S2 = reinterpret_cast<float*>(ws + p.s2_off);

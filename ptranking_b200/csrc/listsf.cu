@@ -138,7 +138,7 @@ int ptrb200_elementwise(int op, const float* a, const float* b, float* out, int6
     if (!a || !out || count <= 0 || op < EW_ADD || op > EW_ACT_GRAD) { set_error("elementwise: bad arguments"); return PTRB200_ERR_INVALID; }
     if (!b && op != EW_RELU && op != EW_DROPOUT && op != EW_ACT && op != EW_ACT_GRAD) { set_error("elementwise: op %d needs two inputs", op); return PTRB200_ERR_INVALID; }
     size_t blocks = ((size_t)count + 255) / 256; if (blocks > (size_t)num_sms() * 16) blocks = (size_t)num_sms() * 16;
-    DropCfg dc = make_drop(dropout_p, seed, offset);
+    DropCfg dc = make_drop_call(dropout_p, seed, offset);
     if (op == EW_ACT || op == EW_ACT_GRAD) dc.thr = (uint32_t)seed;           // seed = PTRB200_AF_* code
     PTRB200_LAUNCH(elementwise_kernel, (unsigned)blocks, 256, 0, stream, op, a, b, out, (size_t)count, dc);
     return check_launch("elementwise");

@@ -127,6 +127,7 @@ TC_CASES = [
     (7, 33, [64, 48, 32, 1], "CE", None, None, False, 0.2),          # no norm, bare last Linear, ragged rows
     (2, 300, [136, 100, 8], "S", "R", "BN", False, 0.0),             # wider output, rows % 128 != 0
     (1, 1, [136, 100, 1], "GE", "S", None, False, 0.0),              # a single document
+    (3, 50, [46, 100, 100, 1], "GE", "S", "BN", True, 0.1),         # 46 features: zero-padded on the tensor cores, same masks
 ]
 
 
