@@ -200,15 +200,22 @@ class ListNeuralRanker(NeuralRanker):
 
     def forward_ragged(self, flat_q_doc_vectors, offsets, max_len, buckets=None):
         """[total_docs, F] + int32 offsets[B+1] -> flat scores [total_docs] for lists of different lengths (the reference can
-        only batch equal-length lists, data_utils.py:683-742).  The batch is padded on the device, the attention masks
-        every query's padded keys (probability exactly 0), all other layers are row-wise, and the scores of the real
-        documents are gathered back -- so each query sees exactly what it would see alone.  With ``buckets``
-        (data.RaggedBatches: the batch sorted by length and cut into length classes) every class is padded to ITS longest
-        list only.  Batch- or list-level normalisation in the head / tail nets would mix padding into its statistics and
-        is refused."""
+        only batch equal-length lists, data_utils.py:683-742).  ``buckets`` (data.RaggedBatches: the batch sorted by length
+        and cut into length classes [(q_begin, q_end, max_len)]) pads every class to ITS longest list only; without them
+        the batch is one class.  The encoder runs on each class padded on the device, its attention masking every query's
+        padded keys (probability exactly 0), so each query's encoder sees exactly what it would see alone.
+
+        Without BN the head and tail nets are row-wise, so the whole scorer runs on the padded blocks and the scores of
+        the real documents are gathered back.  With BN (bn_type 'BN2' or 'BN') padding must not enter a statistic, so the
+        head and tail nets run once each on the flat rows: BN2 normalises every query over its own documents, BN over
+        every real document of the batch -- on an equal-length batch that is the reference's BN over the [B, n] rows.
+        Only the encoder's input is padded, class by class, and its output rows are gathered back into one flat tensor
+        before the DASALC / AllRank / AttnDIN combination.
+
+        Dropout (training) keys its masks by position in the tensor a layer sees: flat row for the head and tail nets on
+        the BN route, padded position for the encoder (and for every layer on the route without BN).  A ragged step
+        therefore draws other masks than processing the queries one by one."""
         cfg = self.sf_para_dict[self.sf_para_dict['sf_id']]
-        if cfg.get('BN', True):
-            raise NotImplementedError("ragged batches through the list scorer need BN=False (the listsf default of the drop-in run)")
         X = flat_q_doc_vectors
         total = X.shape[0]
         offs = offsets.to(device=X.device, dtype=torch.int32).contiguous()
@@ -218,12 +225,37 @@ class ListNeuralRanker(NeuralRanker):
             classes = [(0, B, max(int(max_len), 1))]
         if classes[0][0] != 0 or classes[-1][1] != B or any(a[1] != b[0] for a, b in zip(classes, classes[1:])):
             raise ValueError("buckets must cover the queries of the batch in order")
+        if cfg.get('BN', True):
+            return self._forward_ragged_normalised(X, offs, max_len, classes)
         padded = []
         for q0, q1, nmax in classes:
             sub = offs[q0: q1 + 1]                      # absolute prefix offsets: the kernels index the whole flat batch
             with ops.key_lens_context((sub[1:] - sub[:-1]).contiguous()):
                 padded.append(self.forward(ops.pad_lists(X, sub, nmax)).contiguous())     # [q1 - q0, nmax]
         return ops.unpad_buckets(padded, offs, total, [c[0] for c in classes])
+
+    def _forward_ragged_normalised(self, X, offs, max_len, classes):
+        """forward_ragged with BN / BN2 in the head and tail nets: those run on the flat rows, the encoder per class."""
+        if X.dtype != torch.float32:        # as forward(): the encoder and the glue consume X in fp32
+            X = X.float()
+        head, enc, tail = self.list_sf['head_ffnns'], self.list_sf['encoder'], self.list_sf['tail_ffnns']
+        H = head(X, offsets=offs, max_len=max_len)                          # [total, F]
+        src = X if 'DASALC' == self.encoder_type else H
+        blocks = []
+        for q0, q1, nmax in classes:
+            sub = offs[q0: q1 + 1]
+            with ops.key_lens_context((sub[1:] - sub[:-1]).contiguous()):
+                blocks.append(enc(ops.pad_lists(src, sub, nmax)))           # [q1 - q0, nmax, F]
+        E = ops.unpad_buckets(blocks, offs, X.shape[0], [c[0] for c in classes])   # [total, F]
+        if 'AllRank' == self.encoder_type:
+            z = E
+        elif 'DASALC' == self.encoder_type:
+            z = ops.latent_cross(E, H)
+        elif 'AttnDIN' == self.encoder_type:
+            z = ops.add(E, X)
+        else:
+            raise NotImplementedError
+        return torch.squeeze(tail(z, offsets=offs, max_len=max_len), dim=-1)
 
     def eval_mode(self):
         for part in self.list_sf.values():

@@ -56,7 +56,9 @@ class StackedFFNet(nn.Module):
         computed zero-padded to the next multiple of 4 -- zero weight rows and bias, and for a normalised output layer
         scale 1 / shift 0 -- and the first ff_dims[-1] columns are returned.  The padded columns are constant 0 before
         the norm, so they change neither the other columns' statistics nor their gradients; parameters and checkpoint
-        keys keep their own shapes."""
+        keys keep their own shapes.
+        A ragged per-query BN2 call pads such an output layer in the same way whatever ``pad_output`` says (the list
+        scorer's F-wide head at F = 46); its dense calls keep the kernels they use without padding."""
         super().__init__()
         # "3xtf32" (default): wgmma tensor cores with the fp32-equivalent 3-pass TF32 split;
         # "tf32": single pass; "simt": fp32 FMA kernels (also the fallback for widths the MMA tiles reject)
@@ -99,23 +101,33 @@ class StackedFFNet(nn.Module):
         self.bn_per_query = bool(bn_per_query)
         norm = ("BN2" if bn_per_query else bn_type) if BN else None
         out = ff_dims[-1]
-        self._pad_out = (-out) % 4 if pad_output and out > 4 else 0
-        self.spec = ops.FFNetSpec(list(ff_dims[:-1]) + [out + self._pad_out], AF if L > 2 else None,
-                                  TL_AF if apply_tl_af else None, norm, bn_affine and not bn_per_query, dropout,
-                                  math_mode=math_mode)
+        pad = (-out) % 4 if out > 4 else 0
 
-    def ordered_parameters(self):
+        def spec(padded_out):
+            return ops.FFNetSpec(list(ff_dims[:-1]) + [padded_out], AF if L > 2 else None, TL_AF if apply_tl_af else None,
+                                 norm, bn_affine and not bn_per_query, dropout, math_mode=math_mode)
+        self._pad_out = pad if pad_output else 0
+        self.spec = spec(out + self._pad_out)
+        # ragged per-query statistics run on the tensor-core kernels only, so a ragged BN2 call always pads
+        self._ragged_pad = pad if norm == "BN2" else 0
+        self._ragged_spec = self.spec if self._ragged_pad == self._pad_out else spec(out + self._ragged_pad)
+
+    def ordered_parameters(self, pad=None):
+        """The parameters in the order of the C ABI, with the output layer zero-padded by ``pad`` rows (default: the
+        padding of a dense call)."""
+        pad = self._pad_out if pad is None else pad
         ps = [getattr(getattr(self, e[0]), e[1]) if isinstance(e, tuple) else e for e in self._order]
-        if self._pad_out:
+        if pad:
             # the output layer: weight and bias with zero rows appended, then its norm's (scale, shift) pairs -- gamma
-            # and beta, and BN2's affine weight and bias -- with 1 / 0
+            # and beta, and BN2's affine weight and bias -- with 1 / 0 (BN2 keeps them as [1, 1, width])
             k = self._last
             w = ps[k]
-            ps[k] = torch.cat((w, w.new_zeros(self._pad_out, w.shape[1])))
+            ps[k] = torch.cat((w, w.new_zeros(pad, w.shape[1])))
             for j in range(k + 1, len(ps)):
                 t = ps[j]
-                fill = t.new_ones(self._pad_out) if (j - k) % 2 == 0 else t.new_zeros(self._pad_out)
-                ps[j] = torch.cat((t, fill))
+                shape = (*t.shape[:-1], pad)
+                fill = t.new_ones(shape) if (j - k) % 2 == 0 else t.new_zeros(shape)
+                ps[j] = torch.cat((t, fill), dim=-1)
         return ps
 
     def _grad_targets(self):
@@ -143,17 +155,18 @@ class StackedFFNet(nn.Module):
         squeeze = X.dim() == 2 and not ragged_bn2
         if squeeze:
             X = X.unsqueeze(0)
+        pad = self._ragged_pad if ragged_bn2 else self._pad_out
         # when every parameter already owns gradient storage (the ranker's flat bucket), the backward kernels write
         # into it directly instead of handing autograd 2 tensors per layer to accumulate
         targets = None
-        if torch.is_grad_enabled() and getattr(self, "write_through_grads", False) and not self._pad_out:
+        if torch.is_grad_enabled() and getattr(self, "write_through_grads", False) and not pad:
             targets = self._grad_targets()
         if ragged_bn2:
             if X.dim() != 2:
                 raise ValueError("a ragged batch is [total_docs, F]")
-            out = ops.ffnet_apply(X, self.spec, self.ordered_parameters(), training=self.training, grad_targets=targets,
-                                  offsets=offsets, max_len=max_len)
-            return out[:, :out.shape[1] - self._pad_out].contiguous() if self._pad_out else out
+            out = ops.ffnet_apply(X, self._ragged_spec, self.ordered_parameters(pad), training=self.training,
+                                  grad_targets=targets, offsets=offsets, max_len=max_len)
+            return out[:, :out.shape[1] - pad].contiguous() if pad else out
         out = ops.ffnet_apply(X, self.spec, self.ordered_parameters(), training=self.training, grad_targets=targets)
         if self._pad_out:
             out = out[..., :out.shape[-1] - self._pad_out].contiguous()

@@ -1095,20 +1095,21 @@ class _UnpadLists(torch.autograd.Function):
 
 
 class _UnpadBuckets(torch.autograd.Function):
-    """Padded score blocks of consecutive query ranges -> one flat [total] vector (every block gathers into ITS rows through
-    the absolute prefix offsets); backward pads the gradient block by block."""
+    """Padded blocks [B_k, n_k(, F)] of consecutive query ranges -> one flat [total(, F)] tensor (every block gathers into
+    ITS rows through the absolute prefix offsets); backward pads the gradient block by block."""
 
     @staticmethod
     @_on_tensor_device
     def forward(ctx, offsets, total, q0s, *blocks):
         lib = _lib.load()
         blocks = [_dev_f32(b, "block") for b in blocks]
-        out = torch.empty((total,), dtype=torch.float32, device=blocks[0].device)
+        F = blocks[0].shape[2] if blocks[0].dim() == 3 else 1
+        out = torch.empty((total, F) if blocks[0].dim() == 3 else (total,), dtype=torch.float32, device=blocks[0].device)
         for q0, b in zip(q0s, blocks):
-            _lib.check(lib.ptrb200_unpad_lists(b.data_ptr(), offsets.data_ptr() + 4 * q0, out.data_ptr(), b.shape[0], b.shape[1], 1,
+            _lib.check(lib.ptrb200_unpad_lists(b.data_ptr(), offsets.data_ptr() + 4 * q0, out.data_ptr(), b.shape[0], b.shape[1], F,
                                                _stream_ptr()), "unpad_lists")
         ctx.save_for_backward(offsets)
-        ctx.q0s, ctx.shapes = list(q0s), [tuple(b.shape) for b in blocks]
+        ctx.q0s, ctx.shapes, ctx.F = list(q0s), [tuple(b.shape) for b in blocks], F
         return out
 
     @staticmethod
@@ -1120,15 +1121,19 @@ class _UnpadBuckets(torch.autograd.Function):
         outs = []
         for q0, shp in zip(ctx.q0s, ctx.shapes):
             o = torch.empty(shp, dtype=torch.float32, device=g.device)
-            _lib.check(lib.ptrb200_pad_lists(g.data_ptr(), offsets.data_ptr() + 4 * q0, o.data_ptr(), shp[0], shp[1], 1, _stream_ptr()), "pad_lists")
+            _lib.check(lib.ptrb200_pad_lists(g.data_ptr(), offsets.data_ptr() + 4 * q0, o.data_ptr(), shp[0], shp[1], ctx.F,
+                                             _stream_ptr()), "pad_lists")
             outs.append(o)
         return (None, None, None, *outs)
 
 
 def unpad_buckets(blocks: Sequence[torch.Tensor], offsets: torch.Tensor, total: int, q0s: Sequence[int]) -> torch.Tensor:
-    """Flat [total] scores from padded blocks [B_k, n_k] of consecutive query ranges starting at queries ``q0s``."""
+    """Flat [total] scores (or [total, F] rows) from padded blocks [B_k, n_k] ([B_k, n_k, F]) of consecutive query ranges
+    starting at queries ``q0s``."""
     if sum(b.shape[0] for b in blocks) != offsets.numel() - 1:
         raise ValueError("the blocks must cover every query once")
+    if len({b.shape[2:] for b in blocks}) != 1 or blocks[0].dim() not in (2, 3):
+        raise ValueError("the blocks must all be [B_k, n_k] or all [B_k, n_k, F] with one F")
     return _UnpadBuckets.apply(_offsets_i32(offsets, blocks[0].device), int(total), [int(q) for q in q0s], *blocks)
 
 
