@@ -525,6 +525,61 @@ int ptrb200_tc_gemm_nt(const float* A, const float* B, float* C, int M, int N, i
 int ptrb200_tc_wgrad(const float* dZ, const float* P, float* dW, float* partials, int rows, int N, int K, int passes,
                      ptrb200_stream_t stream);
 
+/* ---- LETOR text files read on the device ------------------------------------------------------------------------ */
+/* LTRDataset's loading path, ptranking/data/data_utils.py:276-549 (iter_lines, parse_letor, iter_queries, clip_query_data),
+ * as six stages; ptranking_b200/letor.py drives them.  `text` is the raw file on the device.  Each stage that sizes a
+ * later buffer reads its sizes back to the host (the *_host arguments) and synchronises `stream`.  A malformed line is
+ * PTRB200_ERR_INVALID with "line <1-based number>: <reason>" in ptrb200_last_error(). */
+#define PTRB200_LETOR_MAX_FEATURES 16384   /* largest feature id + 1 accepted (MSLR 136, Yahoo 700, Istella 220) */
+#define PTRB200_LETOR_NONE      0
+#define PTRB200_LETOR_STANDARD  1          /* sklearn StandardScaler per query */
+#define PTRB200_LETOR_MINMAX    2          /* sklearn MinMaxScaler per query */
+struct ptrb200_letor_cfg {
+    int scaler;            /* PTRB200_LETOR_* */
+    int clip_istella;      /* features clipped at 1e6 before scaling (data_utils.py:483-485) */
+    int rank_labels;       /* MSLETOR_LIST: label r -> n - r (data_utils.py:473-476) */
+    int binary_rele;       /* labels clipped to [-10, 1] */
+    int unknown_as_zero;   /* labels clipped to [0, 10] */
+    int min_docs;          /* a query with fewer documents is dropped (0: no bound) */
+    int min_rele;          /* a query with fewer labels > 0 is dropped (0: no bound) */
+    uint64_t seed;         /* tie shuffle of the presort */
+};
+int64_t ptrb200_letor_index_workspace_bytes(int64_t nbytes);
+/* *n_lines_host = newlines + (1 if the last byte is not a newline) */
+int ptrb200_letor_count_lines(const uint8_t* text, int64_t nbytes, void* workspace, int64_t* n_lines_host, ptrb200_stream_t stream);
+/* line i is text[line_start[i], line_start[i+1] - 1); workspace as left by ptrb200_letor_count_lines */
+int ptrb200_letor_index_lines(const uint8_t* text, int64_t nbytes, const void* workspace, int64_t n_lines, int64_t* line_start,
+                              ptrb200_stream_t stream);
+/* X == NULL: validate every line, write labels[n_lines] (float64, Python float()), qid_span[2 n_lines] (byte offset and
+ * length of the text after "qid:"), info_host[0] = width W (largest feature id + 1 over the file).  X != NULL: write
+ * X[n_lines, W] float64 (absent features 0, a repeated id's last value).  Both: info_host[2] = tokens the exact parser
+ * left undecided (more than 19 significant digits on a rounding boundary); the first undecided_cap of them are listed in
+ * undecided[3 k ..] as (byte offset, length, destination: X index, or -1 - line for a label) for float() on the host.
+ * info: 3 device uint64 of scratch. */
+int ptrb200_letor_parse(const uint8_t* text, const int64_t* line_start, int64_t n_lines, int one_indexed, int has_comment,
+                        double* labels, int64_t* qid_span, double* X, int W, int64_t* undecided, int undecided_cap,
+                        unsigned long long* info, unsigned long long* info_host, ptrb200_stream_t stream);
+int64_t ptrb200_letor_group_workspace_bytes(int64_t n_lines);
+/* Queries by byte-exact qid, in order of first appearance.  offsets == NULL: stats_host[0] = number of queries B.  Then
+ * call again with lines[n_lines], offsets[B+1], counts[B], max_queries = B (same workspace, untouched in between):
+ * lines = line indices grouped per query, in file order within each; stats_host[1] = longest query (an error above
+ * PTRB200_MAX_LIST_LEN). */
+int ptrb200_letor_group(const uint8_t* text, const int64_t* qid_span, int64_t n_lines, void* workspace, int32_t* lines,
+                        int32_t* offsets, int32_t* counts, int max_queries, int* stats_host, ptrb200_stream_t stream);
+/* Labels per query (y[n_lines] fp32, grouped order), clipping and the min_docs / min_rele filter: kept_docs[B] (n or 0),
+ * kept[B] -> rank among kept queries, out_base[B] = first output row; order[n_lines] (optional) = presort order within
+ * each query (ptrb200_shuffle_ties_perm with cfg->seed).  scan_tmp: 2 + 2 * ceil(B / 4096) ints.
+ * stats_host = {kept documents, kept queries}. */
+int ptrb200_letor_select(const double* labels, const int32_t* lines, const int32_t* offsets, int B, int max_len,
+                         const struct ptrb200_letor_cfg* cfg, float* y, int32_t* kept_docs, int32_t* kept, int32_t* out_base,
+                         int32_t* order, int32_t* scan_tmp, int* stats_host, ptrb200_stream_t stream);
+/* Per-query float64 scaling and the output rows: X[total, W] (dtype PTRB200_DTYPE_*), y_out[total],
+ * out_offsets[kept + 1]. */
+int ptrb200_letor_gather(const double* X64, int W, const int32_t* lines, const int32_t* offsets, int B, const int32_t* kept_docs,
+                         const int32_t* kept_rank, const int32_t* out_base, const int32_t* order, const float* y,
+                         const struct ptrb200_letor_cfg* cfg, void* X, int dtype, float* y_out, int32_t* out_offsets,
+                         ptrb200_stream_t stream);
+
 #if defined(__GNUC__)
 #pragma GCC visibility pop
 #endif

@@ -7,6 +7,8 @@
     ptranking_b200.install_diversification()   # DALETOR and DivProbRanker into ptranking.ltr_diversification.eval.ltr_diversification
     DivLTREvaluator(cuda=0).run(model_id='DALETOR', sf_id='pointsf', ...)
 
+    ptranking_b200.install_data()      # opt-in: LTRDataset reads the LETOR files on the device (read_letor)
+
 Importing the package never touches the GPU; the first kernel call loads
 lib/libptranking_b200.so and raises if it (or an sm_90 device) is missing.
 """
@@ -25,6 +27,7 @@ from .ltr_adhoc.listwise.mdprank import MDPRank
 from .ltr_diversification.score_and_sort.daletor import DALETOR
 from .ltr_diversification.score_and_sort.div_prob_ranker import DivProbRanker
 from .base.ranker import LABEL_TYPE
+from .letor import LetorSplit, LTRDataset, read_letor
 
 MODELS = {c.__name__: c for c in (RankNet, LambdaRank, LambdaLoss, ListNet, ListMLE, ApproxNDCG,
                                   RankMSE, RankCosine, STListNet, SoftRank, WassRank, MDPRank)}
@@ -65,4 +68,15 @@ def install_diversification(module=None):
         if hasattr(module, name):
             previous[name] = getattr(module, name)
         setattr(module, name, cls)
+    return previous
+
+
+def install_data(module=None):
+    """Opt-in: make the reference driver load its splits with :class:`ptranking_b200.letor.LTRDataset`, which parses
+    the LETOR files on the device (``LTRDataset(...)`` in ptranking/ltr_adhoc/eval/ltr.py:138-148).  ``install()`` does
+    not call this.  Returns {name: the value it replaced}."""
+    if module is None:
+        import ptranking.ltr_adhoc.eval.ltr as module  # the reference package must be importable
+    previous = {"LTRDataset": getattr(module, "LTRDataset", None)}
+    module.LTRDataset = LTRDataset
     return previous

@@ -116,6 +116,26 @@ SIGNATURES = {
                                       _I, _I, _fp, _I, _I, _U64, _U64, _fp]),
 }
 
+
+
+class LetorCfg(C.Structure):
+    """struct ptrb200_letor_cfg"""
+    _fields_ = [("scaler", C.c_int), ("clip_istella", C.c_int), ("rank_labels", C.c_int), ("binary_rele", C.c_int),
+                ("unknown_as_zero", C.c_int), ("min_docs", C.c_int), ("min_rele", C.c_int), ("seed", C.c_uint64)]
+
+
+_LC = C.POINTER(LetorCfg)
+SIGNATURES.update({
+    "ptrb200_letor_index_workspace_bytes": (_I64, [_I64]),
+    "ptrb200_letor_count_lines": (_I, [_fp, _I64, _fp, C.POINTER(C.c_int64), _fp]),
+    "ptrb200_letor_index_lines": (_I, [_fp, _I64, _fp, _I64, _fp, _fp]),
+    "ptrb200_letor_parse": (_I, [_fp, _fp, _I64, _I, _I, _fp, _fp, _fp, _I, _fp, _I, _fp, C.POINTER(C.c_ulonglong), _fp]),
+    "ptrb200_letor_group_workspace_bytes": (_I64, [_I64]),
+    "ptrb200_letor_group": (_I, [_fp, _fp, _I64, _fp, _fp, _fp, _fp, _I, C.POINTER(C.c_int), _fp]),
+    "ptrb200_letor_select": (_I, [_fp, _fp, _fp, _I, _I, _LC, _fp, _fp, _fp, _fp, _fp, _fp, C.POINTER(C.c_int), _fp]),
+    "ptrb200_letor_gather": (_I, [_fp, _I, _fp, _fp, _I, _fp, _fp, _fp, _fp, _fp, _LC, _fp, _I, _fp, _fp, _fp]),
+})
+
 MAX_PEERS = 16
 
 

@@ -85,6 +85,22 @@ class LengthBucketedBatches:
                 X, y = presort_query(X, y)
             self.buckets[X.shape[0]].append((str(qid), features_to(X, self.feature_dtype), y))
 
+    @classmethod
+    def from_split(cls, split, docs_per_batch: int = 1 << 18, max_queries: Optional[int] = None,
+                   shuffle_seed: Optional[int] = None, drop_ragged: bool = False, rank: int = 0, world: int = 1):
+        """The same batches as the constructor given ``split``'s queries in order, built on the device from a
+        :class:`ptranking_b200.letor.LetorSplit` with no host copy of the features.  The split is taken as read: presort
+        it with ``read_letor(presort=True)``; the feature dtype is the split's."""
+        self = cls([], docs_per_batch=docs_per_batch, max_queries=max_queries, presort=False, shuffle_seed=shuffle_seed,
+                   drop_ragged=drop_ragged, rank=rank, world=world, pin_memory=False,
+                   feature_dtype=split.X.dtype)
+        self.device = split.X.device
+        self.num_features = split.num_features
+        for b in range(len(split)):
+            qid, X, y = split.query(b)
+            self.buckets[X.shape[0]].append((qid, X, y))
+        return self
+
     def batch_size(self, n: int) -> int:
         B = max(1, self.docs_per_batch // n)
         return min(B, self.max_queries) if self.max_queries else B
@@ -115,6 +131,9 @@ class LengthBucketedBatches:
         self.epoch += 1
         for n, members in plan:
             qs = [self.buckets[n][i] for i in members]
+            if getattr(self, "device", None) is not None:        # from_split: the queries are device views
+                yield [q[0] for q in qs], torch.stack([q[1] for q in qs]), torch.stack([q[2] for q in qs])
+                continue
             X = torch.empty((len(qs), n, self.num_features), dtype=self.feature_dtype, pin_memory=self.pin)
             y = torch.empty((len(qs), n), dtype=torch.float32, pin_memory=self.pin)
             for b, (_, Xq, yq) in enumerate(qs):
@@ -207,6 +226,23 @@ class RaggedBatches:
                 X, y = presort_query(X, y)
             self.queries.append((str(qid), features_to(X, self.feature_dtype), y))
 
+    @classmethod
+    def from_split(cls, split, docs_per_batch: int = 1 << 18, max_queries: Optional[int] = None,
+                   shuffle_seed: Optional[int] = None, rank: int = 0, world: int = 1, max_list_len: int = 4096,
+                   bucket_edges: Sequence[int] = (128, 512)):
+        """The same batches as the constructor given ``split``'s queries in order, built on the device from a
+        :class:`ptranking_b200.letor.LetorSplit` with no host copy of the features.  The split is taken as read: presort
+        it with ``read_letor(presort=True)``; the feature dtype is the split's."""
+        self = cls([], docs_per_batch=docs_per_batch, max_queries=max_queries, presort=False, shuffle_seed=shuffle_seed,
+                   rank=rank, world=world, pin_memory=False, max_list_len=max_list_len, bucket_edges=bucket_edges,
+                   feature_dtype=split.X.dtype)
+        if split.max_len > max_list_len:
+            raise ValueError(f"a query of {split.max_len} documents exceeds the per-list kernel limit {max_list_len}")
+        self.device = split.X.device
+        self.num_features = split.num_features
+        self.queries = [split.query(b) for b in range(len(split))]
+        return self
+
     def _plan(self) -> List[List[int]]:
         idx = np.arange(len(self.queries))
         if self.shuffle_seed is not None:
@@ -234,6 +270,12 @@ class RaggedBatches:
             qs = sorted((self.queries[i] for i in members), key=lambda q: -q[1].shape[0])
             lens = np.array([q[1].shape[0] for q in qs], dtype=np.int64)
             total = int(lens.sum())
+            if getattr(self, "device", None) is not None:        # from_split: the queries are device views
+                offsets = torch.zeros(len(qs) + 1, dtype=torch.int32)
+                offsets[1:] = torch.from_numpy(np.cumsum(lens)).to(torch.int32)
+                yield ([q[0] for q in qs], torch.cat([q[1] for q in qs]), torch.cat([q[2] for q in qs]),
+                       offsets.to(self.device), int(lens.max()), length_buckets(lens, edges=self.bucket_edges))
+                continue
             X = torch.empty((total, self.num_features), dtype=self.feature_dtype, pin_memory=self.pin)
             y = torch.empty((total,), dtype=torch.float32, pin_memory=self.pin)
             offsets = torch.zeros(len(qs) + 1, dtype=torch.int32, pin_memory=self.pin)

@@ -58,6 +58,8 @@ def main():
     ap.add_argument("--sf", default="pointsf", choices=["pointsf", "listsf"])
     ap.add_argument("--queries", type=int, default=240)
     ap.add_argument("--keep", action="store_true")
+    ap.add_argument("--gpu-letor", action="store_true",
+                    help="read the LETOR files on the device: ptranking_b200.install_data() replaces the driver's LTRDataset")
     args = ap.parse_args()
 
     work = tempfile.mkdtemp(prefix="dropin_")
@@ -81,6 +83,10 @@ def main():
         cls = getattr(ref_ltr, args.model)
         assert cls.__module__.startswith("ptranking_b200"), cls
         print(f"installed: ptranking.ltr_adhoc.eval.ltr.{args.model} -> {cls.__module__}.{cls.__name__}")
+    if args.gpu_letor:
+        import ptranking_b200
+        ptranking_b200.install_data()
+        print(f"installed: ptranking.ltr_adhoc.eval.ltr.LTRDataset -> {ref_ltr.LTRDataset.__module__}.LTRDataset")
     cuda = None if args.cuda == "none" else int(args.cuda)
     evaluator = LTREvaluator(cuda=cuda)
     t0 = time.time()
