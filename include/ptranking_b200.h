@@ -283,6 +283,27 @@ int ptrb200_pad_lists_pitched(const float* src, long long ld_src, const int32_t*
 int ptrb200_div_list_concat(const float* feats, const float* enc, const int32_t* offsets, const int32_t* qidx, float* out,
                             int B, int n_max, int W, ptrb200_stream_t stream);
 
+/* Rerank mode's first-stage selection, RerankDIVDataset.__getitem__ / deploy_1st_stage_div_discriminating,
+ * ltr_diversification/util/div_data.py:154-192, for every query of a split in one launch sequence.  keys: the
+ * first-stage sort keys, flat [offsets[B]] cut by the B+1 int32 prefix offsets; max_len: the longest list
+ * (<= PTRB200_MAX_LIST_LEN).  Query q keeps the top min(n_q, rerank_k) rows of the total order (key descending, NaN
+ * highest, -0 == +0, then row index ascending).  Outputs: sel_counts[B] = min(n_q, rerank_k), sel_offsets[B+1] their
+ * exclusive scan, and sel_idx[sel_offsets[B]] the kept rows of each query as indices within the query, ascending.
+ * sel_idx needs room for sum_q min(n_q, rerank_k).  total_host (optional, host) receives sel_offsets[B]; passing it
+ * synchronizes the stream.  rerank_k < 1, max_len outside 1..PTRB200_MAX_LIST_LEN or a null pointer is refused. */
+int ptrb200_div_rerank_select(const float* keys, const int32_t* offsets, int B, int max_len, int rerank_k,
+                              int32_t* sel_counts, int32_t* sel_offsets, int32_t* sel_idx, int32_t* total_host,
+                              ptrb200_stream_t stream);
+
+/* The pools of a selection (ptrb200_div_rerank_select), bit-exact copies: docs_out[sel_offsets[q] + j, 0:F] =
+ * docs[(offsets[q] + sel_idx[sel_offsets[q] + j]) * F + 0:F], and query q's subtopic relevance block [m_q, n_q]
+ * (rele_offsets / sub_counts as ptrb200_daletor_fwd_bwd) becomes the [m_q, c_q] block of its selected columns, in
+ * order, at rele_out + rele_offsets_out[q] (int64, written here: the exclusive scan of m_q c_q). */
+int ptrb200_div_rerank_gather(const float* docs, int F, const int32_t* offsets, const int32_t* sel_offsets,
+                              const int32_t* sel_idx, int B, const float* rele, const int64_t* rele_offsets,
+                              const int32_t* sub_counts, float* docs_out, float* rele_out, int64_t* rele_offsets_out,
+                              ptrb200_stream_t stream);
+
 /* ---- stacked feed-forward scorer (pointwise MLP; also the head/tail nets of listsf) ---- */
 /* get_stacked_FFNet, ptranking/base/utils.py:288-356; PointNeuralRanker.forward,
  * base/point_ranker.py:45-55; LTRBatchNorm / LTRBatchNorm2, base/utils.py:201-282;

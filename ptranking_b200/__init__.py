@@ -8,6 +8,7 @@
     DivLTREvaluator(cuda=0).run(model_id='DALETOR', sf_id='pointsf', ...)
 
     ptranking_b200.install_data()      # opt-in: LTRDataset reads the LETOR files on the device (read_letor)
+    ptranking_b200.install_div_rerank()  # opt-in: rerank mode's RerankDIVDataset selects the pools on the device
 
 Importing the package never touches the GPU; the first kernel call loads
 lib/libptranking_b200.so and raises if it (or an sm_90 device) is missing.
@@ -79,4 +80,17 @@ def install_data(module=None):
         import ptranking.ltr_adhoc.eval.ltr as module  # the reference package must be importable
     previous = {"LTRDataset": getattr(module, "LTRDataset", None)}
     module.LTRDataset = LTRDataset
+    return previous
+
+
+def install_div_rerank(module=None):
+    """Opt-in: make the reference's diversification driver wrap its splits in
+    :class:`ptranking_b200.ltr_diversification.div_data.RerankDIVDataset` in rerank mode (``RerankDIVDataset(...)`` in
+    ptranking/ltr_diversification/eval/ltr_diversification.py:62-86), which selects every query's first-stage pool on the
+    device.  ``install_diversification()`` does not call this.  Returns {name: the value it replaced}."""
+    if module is None:
+        import ptranking.ltr_diversification.eval.ltr_diversification as module  # the reference must be importable
+    from .ltr_diversification.div_data import RerankDIVDataset
+    previous = {"RerankDIVDataset": getattr(module, "RerankDIVDataset", None)}
+    module.RerankDIVDataset = RerankDIVDataset
     return previous

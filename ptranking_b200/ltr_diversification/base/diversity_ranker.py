@@ -30,7 +30,8 @@ class _Split:
     list scorer's encoder input), int32 offsets [Q+1] (device) and their host copy, the subtopic relevance blocks, host
     qids / perm_docs and the per-query relevance mass (host, for the skip rules)."""
 
-    def __init__(self, data, device, list_order=False):
+    def __init__(self, data, device, list_order=False, keep_rows=False):
+        """``keep_rows``: also keep the raw rows ``q`` [Q, F] and ``docs`` [total, F] on the device (a rerank pool)."""
         qids, perm_docs, q_reprs, docs, mats = [], [], [], [], []
         for qid, q_repr, q_perm_docs, doc_reprs, _alpha_dcg, _subtopics, q_doc_rele_mat in data:
             qids.append(qid)
@@ -38,17 +39,34 @@ class _Split:
             q_reprs.append(torch.as_tensor(q_repr, dtype=torch.float32).reshape(1, -1))
             docs.append(torch.as_tensor(doc_reprs, dtype=torch.float32))
             mats.append(torch.as_tensor(q_doc_rele_mat, dtype=torch.float32))
-        self.qids, self.perm_docs = qids, perm_docs
         lens = [int(d.shape[0]) for d in docs]
+        rele_sum = np.asarray([float(torch.sum(r)) for r in mats])      # reference's torch.sum, fp32
+        self.sub_counts_host = np.asarray([int(r.shape[0]) for r in mats], dtype=np.int64)
+        q = torch.cat(q_reprs).to(device) if q_reprs else torch.zeros(0, 1, device=device)
+        d = torch.cat(docs).to(device) if docs else torch.zeros(0, 1, device=device)
+        self._setup(qids, perm_docs, q, d, lens, ops.SubtopicRele.pack(mats, device), rele_sum, list_order)
+        if keep_rows:
+            self.q, self.docs = q, d
+
+    @classmethod
+    def from_rows(cls, qids, perm_docs, q, docs, lens, rele, rele_sum, list_order=False):
+        """A split from device rows: q [Q, F], docs [total, F] cut by the host list lengths ``lens``, the relevance
+        blocks ``rele`` (ops.SubtopicRele) and their host relevance mass ``rele_sum`` (a rerank selection)."""
+        sp = cls.__new__(cls)
+        sp._setup(list(qids), list(perm_docs), q, docs, lens, rele, np.asarray(rele_sum, dtype=np.float64), list_order)
+        return sp
+
+    def _setup(self, qids, perm_docs, q, d, lens, rele, rele_sum, list_order):
+        device = d.device
+        self.qids, self.perm_docs = qids, perm_docs
+        lens = [int(n) for n in lens]
         self.offsets_host = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
         self.lens_host = np.asarray(lens, dtype=np.int64)
         self.max_len = max(lens, default=1)
-        self.rele_sum = np.asarray([float(torch.sum(r)) for r in mats])      # reference's torch.sum, fp32
+        self.rele_sum = rele_sum
         self.offsets = torch.from_numpy(self.offsets_host.astype(np.int32)).to(device)
         self.lens = torch.from_numpy(self.lens_host.astype(np.int32)).to(device)
-        self.rele = ops.SubtopicRele.pack(mats, device)
-        q = torch.cat(q_reprs).to(device) if q_reprs else torch.zeros(0, 1, device=device)
-        d = torch.cat(docs).to(device) if docs else torch.zeros(0, 1, device=device)
+        self.rele = rele
         build = ops.div_list_features if list_order else ops.div_features
         self.X = build(q, d, offsets=self.offsets, max_len=self.max_len)
         self._steps, self._plans = {}, {}
@@ -157,9 +175,23 @@ class DiversityNeuralRanker(PointNeuralRanker, DivListNeuralRanker):
         return it), in the split's row order.  The scores themselves by default."""
         return preds
 
+    def split_keys(self, sp):
+        """The sort keys of every row of a packed split from one scorer forward in the ranker's current mode (flat, in
+        the split's row order)."""
+        with torch.no_grad():
+            if 'listsf' == self.sf_id:
+                preds = self.list_scores(sp.X, sp.plan(0, len(sp), self))
+            else:
+                preds = self.div_forward_ragged(sp.X, sp.offsets, sp.max_len)
+            return self.split_sort_keys(preds, sp)
+
     def _split(self, data):
         """The packed device copy of ``data``, built on first use and cached for the dataset object (weakly where the
-        object allows it, so the device copies of a finished fold's splits go with their datasets)."""
+        object allows it, so the device copies of a finished fold's splits go with their datasets).  A rerank dataset
+        (div_data.RerankDIVDataset) selects its pools anew on every call: one pass over the data."""
+        rerank = getattr(data, 'rerank_split', None)
+        if rerank is not None:
+            return rerank(self.device, self.split_list_order())
         try:
             sp = self._weak_splits.get(data)
             if sp is None:
@@ -228,12 +260,7 @@ class DiversityNeuralRanker(PointNeuralRanker, DivListNeuralRanker):
         [, order]) on the device."""
         self.eval_mode()
         sp = self._split(data)
-        with torch.no_grad():
-            if 'listsf' == self.sf_id:
-                preds = self.list_scores(sp.X, sp.plan(0, len(sp), self))
-            else:
-                preds = self.div_forward_ragged(sp.X, sp.offsets, sp.max_len)
-            preds = self.split_sort_keys(preds, sp)
+        preds = self.split_keys(sp)
         res = ops.srd_metrics_at_ks(preds, sp.rele, ks, max_label=1.0 if max_label is None else max_label,
                                     offsets=sp.offsets, max_len=sp.max_len, return_order=return_order)
         return (sp, *res)

@@ -770,6 +770,63 @@ def div_list_features(q_repr: torch.Tensor, docs: torch.Tensor, offsets: Optiona
     return out
 
 
+@_on_tensor_device
+def div_rerank_select(keys: torch.Tensor, offsets: torch.Tensor, max_len: int, rerank_k: int,
+                      total: Optional[int] = None):
+    """Rerank mode's first-stage selection (RerankDIVDataset, div_data.py:154-192) for every query of a split ->
+    (sel_counts [B] int32, sel_offsets [B+1] int32, sel_idx [total] int32): query q keeps its top min(n_q, rerank_k) rows
+    by (key descending, row index ascending), listed as indices within the query in ascending order.  ``keys``: flat
+    [offsets[B]] first-stage sort keys; ``total`` = sum_q min(n_q, rerank_k) when the caller knows it (nothing is read
+    back then), else the total is read back from the device."""
+    lib = _lib.load()
+    k = _dev_f32(keys, "keys")
+    if not (offsets.is_cuda and offsets.device == k.device):
+        raise _lib.B200LibraryError("offsets must live on the device of the keys")
+    offsets = offsets.to(torch.int32).contiguous()
+    B = offsets.numel() - 1
+    counts = torch.empty(max(B, 0), dtype=torch.int32, device=k.device)
+    sel_offsets = torch.empty(max(B, 0) + 1, dtype=torch.int32, device=k.device)
+    cap = total if total is not None else min(k.numel(), max(B, 0) * max(int(rerank_k), 0))
+    sel_idx = torch.empty(max(int(cap), 1), dtype=torch.int32, device=k.device)
+    tot = C.c_int32(0)
+    _lib.check(lib.ptrb200_div_rerank_select(k.data_ptr(), offsets.data_ptr(), B, int(max_len), int(rerank_k),
+                                             counts.data_ptr(), sel_offsets.data_ptr(), sel_idx.data_ptr(),
+                                             None if total is not None else C.byref(tot), _stream_ptr()),
+               "div_rerank_select")
+    return counts, sel_offsets, sel_idx[:int(total if total is not None else tot.value)]
+
+
+@_on_tensor_device
+def div_rerank_gather(docs: torch.Tensor, offsets: torch.Tensor, sel_offsets: torch.Tensor, sel_idx: torch.Tensor,
+                      rele: SubtopicRele, rele_numel: Optional[int] = None):
+    """The pools of a :func:`div_rerank_select` selection, bit-exact copies -> (docs_out [sel_total, F], the selected
+    columns of every query's relevance block as a SubtopicRele).  ``rele_numel`` = sum_q m_q c_q when the caller knows
+    it, else it is read back."""
+    lib = _lib.load()
+    d = _dev_f32(docs, "docs")
+    if d.dim() != 2:
+        raise ValueError(f"expected flat [total_docs, F] documents, got {tuple(d.shape)}")
+    for t, name in ((offsets, "offsets"), (sel_offsets, "sel_offsets"), (sel_idx, "sel_idx")):
+        if t.device != d.device or t.dtype != torch.int32 or not t.is_contiguous():
+            raise ValueError(f"{name} must be a contiguous int32 tensor on {d.device}")
+    B = offsets.numel() - 1
+    if sel_offsets.numel() != B + 1 or rele.sub_counts.numel() != B:
+        raise ValueError(f"{sel_offsets.numel() - 1} selections and {rele.sub_counts.numel()} subtopic blocks for {B} "
+                         f"queries")
+    rp, rop, scp = rele._ptrs(d.device)
+    if rele_numel is None:
+        rele_numel = int(torch.sum(rele.sub_counts.to(torch.int64) * torch.diff(sel_offsets).to(torch.int64)))
+    F = d.shape[1]
+    docs_out = torch.empty((sel_idx.numel(), F), dtype=torch.float32, device=d.device)
+    rele_out = torch.empty(int(rele_numel) + 1, dtype=torch.float32, device=d.device)    # never a null pointer
+    rele_offsets_out = torch.empty(max(B, 0), dtype=torch.int64, device=d.device)
+    _lib.check(lib.ptrb200_div_rerank_gather(d.data_ptr(), F, offsets.data_ptr(), sel_offsets.data_ptr(),
+                                             sel_idx.data_ptr(), B, rp, rop, scp, docs_out.data_ptr(),
+                                             rele_out.data_ptr(), rele_offsets_out.data_ptr(), _stream_ptr()),
+               "div_rerank_gather")
+    return docs_out, SubtopicRele(rele_out, rele_offsets_out, rele.sub_counts, rele.max_sub)
+
+
 def _class_ptrs(offsets: torch.Tensor, qidx: torch.Tensor, device):
     for t, name in ((offsets, "offsets"), (qidx, "qidx")):
         if t.device != device or t.dtype != torch.int32 or not t.is_contiguous():

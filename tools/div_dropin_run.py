@@ -12,6 +12,12 @@ layout the driver reads (load_raw_data, :155-207) -- query_permutation.json, que
 doc_representation.dat, query_doc.json and folder{1..5}/config.yml -- with 100-dimensional representations and
 documents covering 1 to 6 subtopics.  debug=True (5 folds, alpha-nDCG@5 validation), 2 epochs, the pointsf scorer
 by default; ``--sf listsf`` runs the list scorer with the reference's default listsf dict (div_parameter.py:98-104).
+
+``--rerank`` runs rerank mode end to end (ltr_diversification.py:323-335, util/div_data.py:130-192): the driver first
+trains a DivProbRanker first stage (scorer ``--sf``), whose per-fold checkpoints stay where the driver wrote them
+(<dir_run>/Fold-k/, the layout load_pretrained_model and get_opt_model read); the tool writes the rerank_dir JSONs
+that describe it, and the driver then trains and tests DALETOR and DivProbRanker with both scorers on the pools the
+first stage selects (rerank_k = RERANK_K), with ptranking_b200.install_div_rerank() in place for ``--impl b200``.
 """
 import argparse
 import json
@@ -37,6 +43,7 @@ import numpy as np
 np.float = float
 
 EPOCHS = 2
+RERANK_K = 20
 
 
 def write_div_data(root, rng, queries_per_fold=12, F=100):
@@ -78,12 +85,73 @@ def write_div_data(root, rng, queries_per_fold=12, F=100):
             f.write("test_set: [" + ", ".join(str(q) for q in qids) + "]\n")
 
 
+def write_rerank_dir(rerank_dir, sf_para_dict, model_para_dict):
+    """The first stage's scorer and model settings in the JSON layout get_rerank_para_dicts reads
+    (DivScoringFunctionParameter / DivProbRankerParameter with para_json)."""
+    sf_id = sf_para_dict["sf_id"]
+    sf = sf_para_dict[sf_id]
+    if sf_id == "pointsf":
+        body = dict(layers=[sf["num_layers"]], AF=[sf["AF"]], apply_tl_af=[sf["apply_tl_af"]], TL_AF=[sf["TL_AF"]],
+                    BN=[sf["BN"]], bn_type=[sf["bn_type"]], bn_affine=[sf["bn_affine"]])
+    else:
+        body = dict(BN=[sf["BN"]], bn_type=[sf["bn_type"]], bn_affine=[sf["bn_affine"]], ff_dims=sf["ff_dims"],
+                    AF=[sf["AF"]], apply_tl_af=[sf["apply_tl_af"]], TL_AF=[sf["TL_AF"]], n_heads=[sf["n_heads"]],
+                    encoder_type=[sf["encoder_type"]], encoder_layers=[sf["encoder_layers"]])
+    sf_json = {"DivSFParameter": {"sf_id": sf_id, "opt": [sf_para_dict["opt"]], "lr": [sf_para_dict["lr"]], sf_id: body}}
+    with open(os.path.join(rerank_dir, "Div_Data_Eval_ScoringFunction.json"), "w") as f:
+        json.dump(sf_json, f)
+    with open(os.path.join(rerank_dir, "DivProbRankerParameter.json"), "w") as f:
+        json.dump({k: [v] for k, v in model_para_dict.items() if k != "model_id"}, f)
+
+
+def run_rerank(args, ref_div, DivEvalSetting, data_dir, out_dir, work):
+    """First stage, then the four second-stage runs; returns the number of runs that finished."""
+    import torch
+    debug_setting = DivEvalSetting.default_setting
+    rerank = {}
+
+    def with_rerank(self):
+        d = debug_setting(self)
+        d.update(rerank)
+        return d
+    DivEvalSetting.default_setting = with_rerank
+    cuda = None if args.cuda == "none" else int(args.cuda)
+
+    torch.manual_seed(2021)
+    first = ref_div.DivLTREvaluator(cuda=cuda)
+    t0 = time.time()
+    first.run(debug=True, model_id="DivProbRanker", sf_id=args.sf, data_id="WT_Div_0912_Implicit", dir_data=data_dir,
+              dir_output=os.path.join(out_dir, "first_stage") + "/")
+    model_dir = first.dir_run
+    folds = sorted(os.listdir(model_dir))
+    print(f"first stage DivProbRanker ({args.sf}) trained in {time.time() - t0:.1f} s; checkpoints: "
+          + ", ".join(f"{fd}/{os.listdir(os.path.join(model_dir, fd))}" for fd in folds if fd.startswith("Fold-")))
+    rerank_dir = os.path.join(work, "rerank_cfg") + "/"
+    os.makedirs(rerank_dir)
+    write_rerank_dir(rerank_dir, first.sf_parameter.sf_para_dict, first.model_parameter.probrank_para_dict)
+    rerank.update(rerank=True, rerank_k=RERANK_K, rerank_dir=rerank_dir, rerank_model_id="DivProbRanker",
+                  rerank_model_dir=model_dir)
+    done = 0
+    for model_id in ("DALETOR", "DivProbRanker"):
+        for sf_id in ("pointsf", "listsf"):
+            torch.manual_seed(2021)
+            ev = ref_div.DivLTREvaluator(cuda=cuda)
+            print(f"== rerank mode: {model_id} ({sf_id}) on the top {RERANK_K} of the first stage")
+            t0 = time.time()
+            ev.run(debug=True, model_id=model_id, sf_id=sf_id, data_id="WT_Div_0912_Implicit", dir_data=data_dir,
+                   dir_output=os.path.join(out_dir, f"rerank_{model_id}_{sf_id}") + "/")
+            print(f"== {model_id} ({sf_id}) finished in {time.time() - t0:.1f} s (5 folds x {EPOCHS} epochs)")
+            done += 1
+    return done
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--cuda", default="0")
     ap.add_argument("--keep", action="store_true")
     ap.add_argument("--sf", default="pointsf", choices=["pointsf", "listsf"])
+    ap.add_argument("--rerank", action="store_true")
     args = ap.parse_args()
 
     work = tempfile.mkdtemp(prefix="div_dropin_")
@@ -96,12 +164,16 @@ def main():
     import torch
     import ptranking.ltr_diversification.eval.ltr_diversification as ref_div
     from ptranking.ltr_diversification.eval.div_parameter import DivEvalSetting
-    print(f"reference imported from {REF}; impl = {args.impl}; model = DALETOR; scorer = {args.sf}")
+    print(f"reference imported from {REF}; impl = {args.impl}; model = DALETOR; scorer = {args.sf}; "
+          f"rerank = {args.rerank}")
     if args.impl == "b200":
         import ptranking_b200
         ptranking_b200.install_diversification()
         assert ref_div.DALETOR.__module__.startswith("ptranking_b200"), ref_div.DALETOR
         print(f"installed: {ref_div.__name__}.DALETOR -> {ref_div.DALETOR.__module__}.DALETOR")
+        if args.rerank:
+            ptranking_b200.install_div_rerank()
+            print(f"installed: {ref_div.__name__}.RerankDIVDataset -> {ref_div.RerankDIVDataset.__module__}")
 
     # debug=True trains 5 epochs per fold; keep the run short without touching the driver
     debug_setting = DivEvalSetting.default_setting
@@ -112,14 +184,18 @@ def main():
         return d
     DivEvalSetting.default_setting = two_epochs
 
-    torch.manual_seed(2021)
-    cuda = None if args.cuda == "none" else int(args.cuda)
-    evaluator = ref_div.DivLTREvaluator(cuda=cuda)
-    t0 = time.time()
-    evaluator.run(debug=True, model_id="DALETOR", sf_id=args.sf, data_id="WT_Div_0912_Implicit", dir_data=data_dir,
-                  dir_output=out_dir)
-    dt = time.time() - t0
-    print(f"DivLTREvaluator.run finished in {dt:.1f} s (5 folds x {EPOCHS} epochs)")
+    if args.rerank:
+        done = run_rerank(args, ref_div, DivEvalSetting, data_dir, out_dir, work)
+        print(f"rerank mode: {done} of 4 second-stage runs finished")
+    else:
+        torch.manual_seed(2021)
+        cuda = None if args.cuda == "none" else int(args.cuda)
+        evaluator = ref_div.DivLTREvaluator(cuda=cuda)
+        t0 = time.time()
+        evaluator.run(debug=True, model_id="DALETOR", sf_id=args.sf, data_id="WT_Div_0912_Implicit",
+                      dir_data=data_dir, dir_output=out_dir)
+        dt = time.time() - t0
+        print(f"DivLTREvaluator.run finished in {dt:.1f} s (5 folds x {EPOCHS} epochs)")
     if args.impl == "b200":
         from ptranking_b200 import _lib
         print(f"kernels launched by libptranking_b200.so in this process: {_lib.launch_count()}")
