@@ -304,6 +304,29 @@ int ptrb200_div_rerank_gather(const float* docs, int F, const int32_t* offsets, 
                               const int32_t* sub_counts, float* docs_out, float* rele_out, int64_t* rele_offsets_out,
                               ptrb200_stream_t stream);
 
+/* The greedy ideal alpha-DCG order of every query of a split, get_div_ideal_ranking
+ * (metric/srd/diversity_metric.py:113-141), one CTA per query.  Query q's pool is positions 0..n_q-1 of the B+1 int32
+ * prefix offsets (max_len = max n_q <= PTRB200_MAX_LIST_LEN); the subtopics of its position i are
+ * sub_ids[sub_offsets[offsets[q] + i] .. sub_offsets[offsets[q] + i + 1]) (CSR over the split's positions, ids in
+ * 1..20; others are ignored, so refuse them on the host).  pw[c] = (1 - alpha)^c as float64, for c up to the largest
+ * number of subtopic entries of one query.  Each step places the unplaced position with the largest gain
+ * sum_{s of d} pw[count_s] (summed in entry order; ties: the lowest position) and counts its subtopics; once no
+ * unplaced gain is positive the rest follow in pool order.  order[offsets[q] + j] = the position placed j-th. */
+int ptrb200_div_ideal_order(const int32_t* offsets, const int32_t* sub_offsets, const int32_t* sub_ids,
+                            const double* pw, int B, int max_len, int32_t* order, ptrb200_stream_t stream);
+
+/* A split's packed rows in ideal order (DIVDataset, ltr_diversification/util/div_data.py:80-116).  table [D, F] holds
+ * the documents, rows[offsets[q] + i] the table row of query q's pool position i, order the ideal order
+ * (ptrb200_div_ideal_order), sub_offsets / sub_ids its subtopic CSR.  Writes q_out [B, F] = q_src, docs_out[offsets[q]
+ * + j] = table[rows[offsets[q] + order[offsets[q] + j]]] and query q's to_matrix block [m_q, n_q] (m_q = sub_counts[q],
+ * row s-1 = 1 where the document covers subtopic s) at rele_out + rele_offsets[q].  std_delta > 0 adds std_delta times a
+ * standard normal to every q and doc element: Philox4x32-10 keyed by seed, counter (element index, 0 for q_out / 1
+ * for docs_out), so one seed gives bit-identical output.  std_delta must be finite and >= 0. */
+int ptrb200_div_pack_split(const float* table, int F, const float* q_src, const int32_t* offsets, const int32_t* rows,
+                           const int32_t* order, const int32_t* sub_offsets, const int32_t* sub_ids,
+                           const int64_t* rele_offsets, const int32_t* sub_counts, int B, float std_delta,
+                           uint64_t seed, float* q_out, float* docs_out, float* rele_out, ptrb200_stream_t stream);
+
 /* ---- stacked feed-forward scorer (pointwise MLP; also the head/tail nets of listsf) ---- */
 /* get_stacked_FFNet, ptranking/base/utils.py:288-356; PointNeuralRanker.forward,
  * base/point_ranker.py:45-55; LTRBatchNorm / LTRBatchNorm2, base/utils.py:201-282;

@@ -9,6 +9,7 @@
 
     ptranking_b200.install_data()      # opt-in: LTRDataset reads the LETOR files on the device (read_letor)
     ptranking_b200.install_div_rerank()  # opt-in: rerank mode's RerankDIVDataset selects the pools on the device
+    ptranking_b200.install_div_data()  # opt-in: DIVDataset orders and packs every split on the device
 
 Importing the package never touches the GPU; the first kernel call loads
 lib/libptranking_b200.so and raises if it (or an sm_90 device) is missing.
@@ -93,4 +94,18 @@ def install_div_rerank(module=None):
     from .ltr_diversification.div_data import RerankDIVDataset
     previous = {"RerankDIVDataset": getattr(module, "RerankDIVDataset", None)}
     module.RerankDIVDataset = RerankDIVDataset
+    return previous
+
+
+def install_div_data(module=None):
+    """Opt-in: make the reference's diversification driver build its plain splits with
+    :class:`ptranking_b200.ltr_diversification.div_data.DIVDataset` (``DIVDataset(...)`` in
+    ptranking/ltr_diversification/eval/ltr_diversification.py:88-110), which computes the ideal orders and packs the
+    rows on the device.  ``install_diversification()`` does not call this, and rerank mode's RerankDIVDataset keeps
+    building its pool with the reference's class.  Returns {name: the value it replaced}."""
+    if module is None:
+        import ptranking.ltr_diversification.eval.ltr_diversification as module  # the reference must be importable
+    from .ltr_diversification.div_data import DIVDataset
+    previous = {"DIVDataset": getattr(module, "DIVDataset", None)}
+    module.DIVDataset = DIVDataset
     return previous

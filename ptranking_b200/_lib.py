@@ -88,6 +88,8 @@ SIGNATURES = {
     "ptrb200_div_list_concat": (_I, [_fp, _fp, _fp, _fp, _fp, _I, _I, _I, _fp]),
     "ptrb200_div_rerank_select": (_I, [_fp, _fp, _I, _I, _I, _fp, _fp, _fp, C.POINTER(C.c_int32), _fp]),
     "ptrb200_div_rerank_gather": (_I, [_fp, _I, _fp, _fp, _fp, _I, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
+    "ptrb200_div_ideal_order": (_I, [_fp, _fp, _fp, _fp, _I, _I, _fp, _fp]),
+    "ptrb200_div_pack_split": (_I, [_fp, _I, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _I, _F, _U64, _fp, _fp, _fp, _fp]),
     "ptrb200_standard_scale": (_I, [_fp, _fp, _fp, _I, _I, _I, _I, _F, _fp]),
     "ptrb200_sum_f32": (_I, [_fp, _fp, _I, _fp]),
     "ptrb200_ndcg_at_ks": (_I, [_fp, _fp, _fp, C.POINTER(C.c_int32), _I, _fp, _fp, _I, _I, _I, _fp]),

@@ -16,27 +16,6 @@ constexpr int RR_SELECT_THREADS = 256;
 constexpr int RR_SCAN_THREADS = 1024;
 constexpr int RR_GATHER_THREADS = 256, RR_GATHER_Y = 4;
 
-// Block-wide exclusive scan; every thread gets its prefix and *total.  `red` = 64 elements of shared memory.
-template <typename T>
-static __device__ __forceinline__ T rr_block_exclusive_scan(T v, T* red, T* total) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    T inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const T t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
-    __syncthreads();
-    if (lane == 31) red[warp] = inc;
-    __syncthreads();
-    if (warp == 0) {
-        T s = lane < nw ? red[lane] : T(0);
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const T t = __shfl_up_sync(0xffffffffu, s, o); if (lane >= o) s += t; }
-        red[32 + lane] = s;
-    }
-    __syncthreads();
-    *total = red[32 + nw - 1];
-    return inc - v + (warp ? red[32 + warp - 1] : T(0));
-}
-
 __global__ void __launch_bounds__(RR_SCAN_THREADS)
 rerank_count_scan_kernel(const int32_t* __restrict__ offsets, int B, int k, int32_t* __restrict__ counts,
                          int32_t* __restrict__ sel_offsets) {
@@ -46,7 +25,7 @@ rerank_count_scan_kernel(const int32_t* __restrict__ offsets, int B, int k, int3
         const int q = q0 + threadIdx.x;
         const int32_t c = q < B ? max(0, min(offsets[q + 1] - offsets[q], k)) : 0;
         int32_t tot;
-        const int32_t ex = rr_block_exclusive_scan(c, red, &tot);
+        const int32_t ex = block_exclusive_scan(c, red, &tot);
         if (q < B) { counts[q] = c; sel_offsets[q] = carry + ex; }
         carry += tot;
     }
@@ -62,7 +41,7 @@ rerank_rele_scan_kernel(const int32_t* __restrict__ sel_offsets, const int32_t* 
         const int q = q0 + threadIdx.x;
         const int64_t c = q < B ? (int64_t)sub_counts[q] * (int64_t)(sel_offsets[q + 1] - sel_offsets[q]) : 0;
         int64_t tot;
-        const int64_t ex = rr_block_exclusive_scan(c, red, &tot);
+        const int64_t ex = block_exclusive_scan(c, red, &tot);
         if (q < B) out[q] = carry + ex;
         carry += tot;
     }
@@ -96,7 +75,7 @@ rerank_select_kernel(const float* __restrict__ keys, const int32_t* __restrict__
     int32_t c = 0;
     for (int r = r0; r < r1; ++r) c += win[r];
     int32_t tot;
-    int32_t pos = rr_block_exclusive_scan(c, red, &tot);
+    int32_t pos = block_exclusive_scan(c, red, &tot);
     for (int r = r0; r < r1; ++r)
         if (win[r]) out[pos++] = r;
 }

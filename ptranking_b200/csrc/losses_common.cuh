@@ -88,6 +88,27 @@ static __device__ void block_scan_inclusive(float* a, int n, float* red /* >= 66
     __syncthreads();
 }
 
+// Block-wide exclusive scan; every thread gets its prefix and *total.  `red` = 64 elements of shared memory.
+template <typename T>
+static __device__ __forceinline__ T block_exclusive_scan(T v, T* red, T* total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    T inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const T t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
+    __syncthreads();
+    if (lane == 31) red[warp] = inc;
+    __syncthreads();
+    if (warp == 0) {
+        T s = lane < nw ? red[lane] : T(0);
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const T t = __shfl_up_sync(0xffffffffu, s, o); if (lane >= o) s += t; }
+        red[32 + lane] = s;
+    }
+    __syncthreads();
+    *total = red[32 + nw - 1];
+    return inc - v + (warp ? red[32 + warp - 1] : T(0));
+}
+
 // ---------------------------------------------------------------------------
 // host-side launch helpers
 // ---------------------------------------------------------------------------

@@ -188,14 +188,18 @@ class DiversityNeuralRanker(PointNeuralRanker, DivListNeuralRanker):
     def _split(self, data):
         """The packed device copy of ``data``, built on first use and cached for the dataset object (weakly where the
         object allows it, so the device copies of a finished fold's splits go with their datasets).  A rerank dataset
-        (div_data.RerankDIVDataset) selects its pools anew on every call: one pass over the data."""
+        (div_data.RerankDIVDataset) selects its pools anew on every call: one pass over the data.  A device-built
+        dataset (div_data.DIVDataset) hands over its packed rows as they are."""
         rerank = getattr(data, 'rerank_split', None)
         if rerank is not None:
             return rerank(self.device, self.split_list_order())
         try:
             sp = self._weak_splits.get(data)
             if sp is None:
-                sp = self._weak_splits[data] = _Split(data, self.device, self.split_list_order())
+                device_split = getattr(data, 'device_split', None)
+                sp = self._weak_splits[data] = (_Split(data, self.device, self.split_list_order())
+                                                if device_split is None
+                                                else device_split(self.device, self.split_list_order()))
             return sp
         except TypeError:                           # e.g. a plain list of query tuples
             hit = self._splits.get(id(data))

@@ -827,6 +827,65 @@ def div_rerank_gather(docs: torch.Tensor, offsets: torch.Tensor, sel_offsets: to
     return docs_out, SubtopicRele(rele_out, rele_offsets_out, rele.sub_counts, rele.max_sub)
 
 
+def _check_i32(device, **named):
+    for name, t in named.items():
+        if not t.is_cuda or t.device != device or t.dtype != torch.int32 or not t.is_contiguous():
+            raise ValueError(f"{name} must be a contiguous int32 tensor on {device}")
+
+
+@_on_tensor_device
+def div_ideal_order(offsets: torch.Tensor, sub_offsets: torch.Tensor, sub_ids: torch.Tensor, pw: torch.Tensor,
+                    max_len: int) -> torch.Tensor:
+    """The greedy ideal alpha-DCG order (get_div_ideal_ranking) of every query of a split -> int32 [offsets[B]]: for
+    query q, order[offsets[q] + j] is the pool position placed j-th.  ``sub_offsets`` [offsets[B] + 1] / ``sub_ids``
+    (1..20): the subtopic CSR over the split's pool positions; ``pw`` float64 (1 - alpha)^c for c = 0 .. the largest
+    number of subtopic entries of one query.  Ties go to the lower pool position."""
+    lib = _lib.load()
+    dev = offsets.device
+    _check_i32(dev, offsets=offsets, sub_offsets=sub_offsets, sub_ids=sub_ids)
+    if not (pw.is_cuda and pw.device == dev and pw.dtype == torch.float64 and pw.is_contiguous()):
+        raise ValueError(f"pw must be a contiguous float64 tensor on {dev}")
+    B = offsets.numel() - 1
+    order = torch.empty(max(sub_offsets.numel() - 1, 1), dtype=torch.int32, device=dev)
+    _lib.check(lib.ptrb200_div_ideal_order(offsets.data_ptr(), sub_offsets.data_ptr(), sub_ids.data_ptr(),
+                                           pw.data_ptr(), B, int(max_len), order.data_ptr(), _stream_ptr()),
+               "div_ideal_order")
+    return order[:sub_offsets.numel() - 1]
+
+
+@_on_tensor_device
+def div_pack_split(table: torch.Tensor, q_src: torch.Tensor, offsets: torch.Tensor, rows: torch.Tensor,
+                   order: torch.Tensor, sub_offsets: torch.Tensor, sub_ids: torch.Tensor, rele_offsets: torch.Tensor,
+                   sub_counts: torch.Tensor, rele_numel: int, max_sub: int, std_delta: float = 0.0, seed: int = 0):
+    """A split's rows in ideal order (DIVDataset) -> (q [B, F], docs [offsets[B], F], SubtopicRele of the to_matrix
+    blocks).  ``table`` [D, F] fp32 documents, ``rows`` the table row of every pool position, ``order`` from
+    :func:`div_ideal_order`, ``rele_offsets`` (int64) / ``sub_counts`` (int32) the blocks' layout, ``rele_numel`` its
+    total size and ``max_sub`` max m_q (host).  ``std_delta`` > 0 adds N(0, std_delta^2) noise keyed by ``seed``."""
+    lib = _lib.load()
+    t = _dev_f32(table, "table")
+    qs = _dev_f32(q_src, "q_src")
+    if t.dim() != 2 or qs.dim() != 2 or qs.shape[1] != t.shape[1]:
+        raise ValueError(f"expected table [D, F] and q_src [B, F], got {tuple(t.shape)} and {tuple(qs.shape)}")
+    dev = t.device
+    _check_i32(dev, offsets=offsets, rows=rows, order=order, sub_offsets=sub_offsets, sub_ids=sub_ids,
+               sub_counts=sub_counts)
+    if rele_offsets.device != dev or rele_offsets.dtype != torch.int64 or not rele_offsets.is_contiguous():
+        raise ValueError(f"rele_offsets must be a contiguous int64 tensor on {dev}")
+    B, F = offsets.numel() - 1, t.shape[1]
+    if qs.shape[0] != B or sub_counts.numel() != B or rele_offsets.numel() != B:
+        raise ValueError(f"{qs.shape[0]} query rows, {sub_counts.numel()} blocks for {B} queries")
+    q_out = torch.empty((B, F), dtype=torch.float32, device=dev)
+    docs_out = torch.empty((rows.numel(), F), dtype=torch.float32, device=dev)
+    rele_out = torch.empty(int(rele_numel) + 1, dtype=torch.float32, device=dev)    # never a null pointer
+    _lib.check(lib.ptrb200_div_pack_split(t.data_ptr(), F, qs.data_ptr(), offsets.data_ptr(), rows.data_ptr(),
+                                          order.data_ptr(), sub_offsets.data_ptr(), sub_ids.data_ptr(),
+                                          rele_offsets.data_ptr(), sub_counts.data_ptr(), B, float(std_delta),
+                                          int(seed) & (2 ** 64 - 1), q_out.data_ptr(), docs_out.data_ptr(),
+                                          rele_out.data_ptr(), _stream_ptr()),
+               "div_pack_split")
+    return q_out, docs_out, SubtopicRele(rele_out, rele_offsets, sub_counts, max_sub)
+
+
 def _class_ptrs(offsets: torch.Tensor, qidx: torch.Tensor, device):
     for t, name in ((offsets, "offsets"), (qidx, "qidx")):
         if t.device != device or t.dtype != torch.int32 or not t.is_contiguous():

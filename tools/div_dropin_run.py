@@ -13,6 +13,9 @@ doc_representation.dat, query_doc.json and folder{1..5}/config.yml -- with 100-d
 documents covering 1 to 6 subtopics.  debug=True (5 folds, alpha-nDCG@5 validation), 2 epochs, the pointsf scorer
 by default; ``--sf listsf`` runs the list scorer with the reference's default listsf dict (div_parameter.py:98-104).
 
+``--model DivProbRanker`` trains DivProbRanker instead.  ``--gpu-data`` (with ``--impl b200``) builds the plain splits
+with the device DIVDataset through ptranking_b200.install_div_data().
+
 ``--rerank`` runs rerank mode end to end (ltr_diversification.py:323-335, util/div_data.py:130-192): the driver first
 trains a DivProbRanker first stage (scorer ``--sf``), whose per-fold checkpoints stay where the driver wrote them
 (<dir_run>/Fold-k/, the layout load_pretrained_model and get_opt_model read); the tool writes the rerank_dir JSONs
@@ -151,7 +154,10 @@ def main():
     ap.add_argument("--cuda", default="0")
     ap.add_argument("--keep", action="store_true")
     ap.add_argument("--sf", default="pointsf", choices=["pointsf", "listsf"])
+    ap.add_argument("--model", default="DALETOR", choices=["DALETOR", "DivProbRanker"])
     ap.add_argument("--rerank", action="store_true")
+    ap.add_argument("--gpu-data", action="store_true",
+                    help="build the plain splits with the device DIVDataset (ptranking_b200.install_div_data())")
     args = ap.parse_args()
 
     work = tempfile.mkdtemp(prefix="div_dropin_")
@@ -164,8 +170,8 @@ def main():
     import torch
     import ptranking.ltr_diversification.eval.ltr_diversification as ref_div
     from ptranking.ltr_diversification.eval.div_parameter import DivEvalSetting
-    print(f"reference imported from {REF}; impl = {args.impl}; model = DALETOR; scorer = {args.sf}; "
-          f"rerank = {args.rerank}")
+    print(f"reference imported from {REF}; impl = {args.impl}; model = {args.model}; scorer = {args.sf}; "
+          f"rerank = {args.rerank}; device DIVDataset = {args.gpu_data}")
     if args.impl == "b200":
         import ptranking_b200
         ptranking_b200.install_diversification()
@@ -174,6 +180,9 @@ def main():
         if args.rerank:
             ptranking_b200.install_div_rerank()
             print(f"installed: {ref_div.__name__}.RerankDIVDataset -> {ref_div.RerankDIVDataset.__module__}")
+        if args.gpu_data:
+            ptranking_b200.install_div_data()
+            print(f"installed: {ref_div.__name__}.DIVDataset -> {ref_div.DIVDataset.__module__}")
 
     # debug=True trains 5 epochs per fold; keep the run short without touching the driver
     debug_setting = DivEvalSetting.default_setting
@@ -192,7 +201,7 @@ def main():
         cuda = None if args.cuda == "none" else int(args.cuda)
         evaluator = ref_div.DivLTREvaluator(cuda=cuda)
         t0 = time.time()
-        evaluator.run(debug=True, model_id="DALETOR", sf_id=args.sf, data_id="WT_Div_0912_Implicit",
+        evaluator.run(debug=True, model_id=args.model, sf_id=args.sf, data_id="WT_Div_0912_Implicit",
                       dir_data=data_dir, dir_output=out_dir)
         dt = time.time() - t0
         print(f"DivLTREvaluator.run finished in {dt:.1f} s (5 folds x {EPOCHS} epochs)")
