@@ -911,16 +911,19 @@ constexpr int WG_MAX_STAGES = 4;      // raw-tile ring depth bound (TMA bulk cop
 
 // Persistent and TMA-fed.  Row tiles of dZ and of the layer input are contiguous in HBM, so warp 0 streams them into
 // a raw shared-memory ring with 1-D bulk copies (cp.async.bulk + mbarrier complete_tx) `stages` tiles ahead.  All
-// threads turn a raw tile into transposed hi/lo TF32 operand buffers (double buffered); the MMAs of a tile run
-// asynchronously while the next tile is staged.  Warpgroup w multiplies dZ columns [64 (w & 1), +64) by the input
-// columns of half (w >> 1) of the block.
+// threads turn a raw tile into transposed hi/lo TF32 operand buffers (double buffered).  A tile's MMAs are committed
+// without a wait and run while the next tile is staged into the other buffer; each thread waits for its warpgroup's
+// MMAs only after that staging, and the CTA barrier behind the wait frees the buffer they read for the tile after.
+// Warpgroup w multiplies dZ columns [64 (w & 1), +64) by the input columns of half (w >> 1) of the block.
 // XB: g.P holds bf16 features (layer 0).  The raw ring carries them at 2 bytes each and the staging widens them while
 // transposing.  A bulk copy needs 16-byte sizes and addresses; a P tile (or, column-blocked, a row segment) that does not
 // have them is copied by hand, as odd-sized dZ tiles are.
 template <int PASSES, bool XB = false>
 __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(WgradArgs g) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    // aligned up by an offset from smem_raw (not through an integer cast of the pointer), so the compiler still knows
+    // every buffer below is shared memory and stages the operands with LDS / STS instead of generic loads and stores
+    unsigned char* base = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
     const int R = g.tile_rows;
     // column block of this CTA: dZ columns [m0, m0+N), layer-input columns [kk0, kk0+K)
     const int m0 = blockIdx.y * 128, kk0 = blockIdx.z * g.kb;
@@ -1025,12 +1028,24 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(WgradArgs g) {
     // computes but does not write), so no operand row beyond KP is read
     const int mh = wg & 1, KPh = ((KP / 16 + 1) / 2) * 16, c0 = (wg >> 1) ? KP - KPh : 0, cw0 = (wg >> 1) ? KPh : 0;
     const int RQ = R / 4;                                    // 16-byte units (4 rows r) per operand row
+    // a thread stages dZ^T column n = tid & 127 of every tile (its units u = tid + 512 j, and 512 % 128 == 0), so the one
+    // statistics group's coefficients of that column stay in registers
+    const float k1n = single_group ? coef[tid & 127] : 0.0f, k3n = single_group ? coef[128 + (tid & 127)] : 0.0f,
+                k0n = single_group ? coef[256 + (tid & 127)] : 0.0f;
+    // the layer-input units of a thread, u = tid + 512 j, as (u % KP, u / KP): stepped instead of divided at every unit
+    const int pk0 = tid % KP, pq0 = tid / KP, pkstep = WG_THREADS % KP, pqstep = WG_THREADS / KP;
 
     tc::with_width(KPh, [&](auto W) {
     constexpr int NPc = decltype(W)::value;
     float acc[NPc / 2];
 #pragma unroll
     for (int e = 0; e < NPc / 2; ++e) acc[e] = 0.0f;
+    // pins the accumulators in place while MMAs run asynchronously over the staging code (no copies of them in between)
+    auto fence_acc = [&]() {
+#pragma unroll
+        for (int e = 0; e < NPc / 2; ++e) asm volatile("" : "+f"(acc[e])::"memory");
+    };
+    fence_acc();
     for (int it = 0; it < my_tiles; ++it) {
         const int t = blockIdx.x + it * gridDim.x, o = it & 1, s = it % stages;
         const int row0 = t * R, nrows = min(R, g.rows - row0);
@@ -1069,7 +1084,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(WgradArgs g) {
                     if (fused_dz) {                                  // host guarantees N % 4 == 0 here
                         const float z = rz[rawz1 / 4 + r * N + n];
                         float a1, a3, a0;
-                        if (single_group) { a1 = coef[n]; a3 = coef[128 + n]; a0 = coef[256 + n]; }
+                        if (single_group) { a1 = k1n; a3 = k3n; a0 = k0n; }
                         else {
                             const size_t go = (size_t)((row0 + r) / g.gr_cur) * g.N_full + grp_off_base;
                             a1 = __ldg(g.kc1 + go); a3 = __ldg(g.kc3 + go); a0 = __ldg(g.kc0 + go);
@@ -1082,8 +1097,8 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(WgradArgs g) {
             put(zh, zl, tc::swz_offset(n, qq), make_float4(v[0], v[1], v[2], v[3]));
         }
         // ---- layer input^T: unit (k, q) = Ain[4q .. 4q+3][k] ----
-        for (int u = tid; u < KP * RQ; u += WG_THREADS) {
-            const int k = u % KP, qq = u / KP;
+        for (int u = tid, k = pk0, qq = pq0; u < KP * RQ; u += WG_THREADS, k += pkstep, qq += pqstep) {
+            if (k >= KP) { k -= KP; ++qq; }                 // (k, qq) = (u % KP, u / KP)
             if (k >= K) continue;
             float v[4];
 #pragma unroll
@@ -1107,6 +1122,10 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(WgradArgs g) {
             }
             put(ph, pl, tc::swz_offset(k, qq), make_float4(v[0], v[1], v[2], v[3]));
         }
+        // Tile it-1's MMAs ran while this tile was staged.  Once every warpgroup has waited for its own and passed the
+        // barrier, operand buffer o ^ 1 -- which all four warpgroups read -- is free for tile it+1.
+        tc::wg_wait<0>();
+        fence_acc();
         tc::fence_proxy_async();
         __syncthreads();
         if (warp == 0 && it + stages < my_tiles) issue_load(it + stages, s);   // raw slot s is drained
@@ -1124,8 +1143,10 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc_kernel(WgradArgs g) {
             tc::mma_tf32<NPc>(acc, ah + 2 * st, bh + 2 * st, 1u);
         }
         tc::wg_commit();
-        tc::wg_wait<0>();                                    // the same threads stage the next tile
+        fence_acc();
     }
+    tc::wg_wait<0>();
+    fence_acc();
     // ---- epilogue: this CTA's partial dW[n][k] ----
     float* dst = g.partials + (size_t)blockIdx.x * g.N_full * g.K_full + (size_t)m0 * g.K_full + kk0;
 #pragma unroll
