@@ -191,13 +191,11 @@ int ptrb200_adhoc_metrics_at_ks(const float* scores, const float* labels, const 
  * (ptranking/data/data_utils.py:482-487; selection :205-218): out = (x - mean_q) / std_q per feature column with the
  * population standard deviation, statistics in float64, constant columns divided by 1.  X/out: [B,n,F] dense, or flat
  * [offsets[B], F] with per-query offsets (ragged).  clip != 0 first clamps features at clip_max (the ISTELLA_MAX clip,
- * :484-485).  In-place (out == X) is allowed. */
-int ptrb200_standard_scale(const float* X, const int32_t* offsets, float* out, int B, int n, int F,
+ * :484-485).  out_dtype (PTRB200_DTYPE_*) is the element type of `out`: F32 may run in place (out == X); BF16 (raw bf16
+ * bit patterns) is the fp32 result rounded to nearest even at the store -- scaling first, because raw LETOR features
+ * lose precision in bf16 -- and must not alias X.  An unknown out_dtype returns PTRB200_ERR_INVALID. */
+int ptrb200_standard_scale(const float* X, const int32_t* offsets, void* out, int out_dtype, int B, int n, int F,
                            int clip, float clip_max, ptrb200_stream_t stream);
-/* The same with bf16 output (raw bf16 bit patterns): the result is computed exactly as above in fp32 and rounded to nearest
- * even at the store -- scaling first, because raw LETOR features lose precision in bf16.  out must not alias X. */
-int ptrb200_standard_scale_bf16(const float* X, const int32_t* offsets, uint16_t* out, int B, int n, int F,
-                                int clip, float clip_max, ptrb200_stream_t stream);
 
 /* ---- search-result diversification (ptranking/ltr_diversification/) ----------------------------------- */
 /* Subtopic relevance of a ragged batch: query q's q_doc_rele_mat is a dense row-major [sub_counts[q], n_q] fp32 block
@@ -273,13 +271,9 @@ int ptrb200_div_list_features(const float* q_repr, const float* docs, const int3
 
 /* One length class of a ragged batch (flat rows cut by the B_all+1 int32 prefix offsets): class query b is query qidx[b]
  * (qidx: B int32 on the device, or NULL for queries 0..B-1), every list of the class has at most n_max rows.
- * ptrb200_pad_lists_pitched: padded[b, r, 0:W] = src[(offsets[q] + r) * ld_src + 0:W] for the list's rows, 0 behind
- * them -- a strided column block of the rows (ld_src >= W) into the dense [B, n_max, W] layout of the encoder.
  * ptrb200_div_list_concat: the uni_sf input of the class's rows, div_list_ranker.py:80: out[row, 0:W] = feats[row, 0:W]
  * and out[row, W:2W] = enc[b, r, 0:W] (enc: the encoder's padded [B, n_max, W] output; out rows are 2W wide).  Its
- * backward is ptrb200_pad_lists_pitched on columns W:2W of the gradient (src = grad + W, ld_src = 2W). */
-int ptrb200_pad_lists_pitched(const float* src, long long ld_src, const int32_t* offsets, const int32_t* qidx,
-                              float* padded, int B, int n_max, int W, ptrb200_stream_t stream);
+ * backward is ptrb200_pad_lists on columns W:2W of the gradient (src = grad + W, ld_src = 2W). */
 int ptrb200_div_list_concat(const float* feats, const float* enc, const int32_t* offsets, const int32_t* qidx, float* out,
                             int B, int n_max, int W, ptrb200_stream_t stream);
 
@@ -352,13 +346,14 @@ int ptrb200_div_pack_split(const float* table, int F, const float* q_src, const 
                                    (round-to-nearest-even), products exact, fp32 accumulation: the numerics of a bf16
                                    tensor-core GEMM, issued as one tf32 wgmma pass (bf16 values are tf32 values).
                                    Activations, weights and the workspace stay fp32 in memory; the features may be
-                                   bf16 in memory (the _x entries below, PTRB200_DTYPE_BF16), which halves their
-                                   reads.  Needs tensor-core-eligible widths (no SIMT fallback) */
+                                   bf16 in memory (x_dtype PTRB200_DTYPE_BF16 below), which halves their reads.
+                                   Needs tensor-core-eligible widths (no SIMT fallback) */
 
-/* Element type of the feature matrix X in the ptrb200_ffnet_*_x entries.  A bf16 X gives bit for bit the results of the
- * same values passed as fp32 (bf16 values are exact in fp32 and tf32), in every math mode. */
+/* Element types: of the feature matrix X of the ptrb200_ffnet_* calls (x_dtype), and of the output of
+ * ptrb200_standard_scale and ptrb200_letor_gather.  A bf16 X gives bit for bit the results of the same values passed as
+ * fp32 (bf16 values are exact in fp32 and tf32), in every math mode. */
 #define PTRB200_DTYPE_F32  0
-#define PTRB200_DTYPE_BF16 1   /* raw bf16 bit patterns, 8-byte aligned, row pitch dims[0] elements */
+#define PTRB200_DTYPE_BF16 1   /* raw bf16 bit patterns; a feature matrix X: 8-byte aligned, row pitch dims[0] elements */
 
 typedef struct ptrb200_ffnet {
     int num_linear;                        /* linear layers, output layer included            */
@@ -409,8 +404,13 @@ int ptrb200_set_hook(ptrb200_hook_fn fn, void* user);
  * offsets[B+1], n = the longest list, X is [total_rows, dims[0]].  Batch-level BN and norm-free nets treat a ragged batch as
  * one long list; per-query BN2 (LTRBatchNorm2) normalises every query over its own documents. */
 
-/* bytes of activation workspace the forward pass fills for the backward pass */
-int64_t ptrb200_ffnet_workspace_bytes(const ptrb200_ffnet* net, int B, int n, int total_rows);
+/* The feature element type X of the three calls is x_dtype (PTRB200_DTYPE_*).  A bf16 X is read natively by layer 0's
+ * tensor-core kernels (forward and weight gradient, half the feature bytes, no fp32 copy); a feature width that is not a
+ * multiple of 4 and math_mode SIMT widen it once into the workspace instead.  dX stays fp32.  An unknown x_dtype or a
+ * bf16 X that is not 8-byte aligned returns PTRB200_ERR_INVALID. */
+
+/* bytes of activation workspace the forward pass fills for the backward pass (it depends on x_dtype) */
+int64_t ptrb200_ffnet_workspace_bytes(const ptrb200_ffnet* net, int x_dtype, int B, int n, int total_rows);
 
 /* `training` argument of the two calls below: bit 0 = training mode (dropout active); bit 1 (forward only) tells
  * ptrb200_ffnet_forward that no backward call will follow, so the by-products the backward pass reads are not written. */
@@ -418,30 +418,16 @@ int64_t ptrb200_ffnet_workspace_bytes(const ptrb200_ffnet* net, int B, int n, in
 #define PTRB200_FFNET_FORWARD_ONLY 2
 /* forward: X[B,n,dims[0]] -> out[B,n,dims[last]].  `workspace` keeps pre-activations and
  * statistics for ptrb200_ffnet_backward.  dropout uses Philox keyed by (seed, offset). */
-int ptrb200_ffnet_forward(const ptrb200_ffnet* net, const float* X, float* out, void* workspace,
+int ptrb200_ffnet_forward(const ptrb200_ffnet* net, const void* X, int x_dtype, float* out, void* workspace,
                           int64_t workspace_bytes, int B, int n, const int32_t* offsets, int total_rows, int training,
                           uint64_t seed, uint64_t offset, ptrb200_stream_t stream);
 
 /* backward: dOut[B,n,dims[last]] -> parameter grads (+ dX[B,n,dims[0]] when dX != NULL).
- * Must follow a forward call with the same net/X/workspace/seed/offset. */
-int ptrb200_ffnet_backward(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, const float* X,
+ * Must follow a forward call with the same net/X/x_dtype/workspace/seed/offset. */
+int ptrb200_ffnet_backward(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, const void* X, int x_dtype,
                            const float* dOut, float* dX, void* workspace, int64_t workspace_bytes,
                            int B, int n, const int32_t* offsets, int total_rows, int training, uint64_t seed, uint64_t offset,
                            ptrb200_stream_t stream);
-
-/* The three calls above with the feature element type as an argument (x_dtype = PTRB200_DTYPE_*; the calls above are
- * these with PTRB200_DTYPE_F32).  A bf16 X is read natively by layer 0's tensor-core kernels (forward and weight
- * gradient, half the feature bytes, no fp32 copy); a feature width that is not a multiple of 4 and math_mode SIMT widen
- * it once into the workspace instead.  dX stays fp32.  An unknown x_dtype or a bf16 X that is not 8-byte aligned returns
- * PTRB200_ERR_INVALID.  The workspace size depends on x_dtype: size it with the _x call. */
-int64_t ptrb200_ffnet_workspace_bytes_x(const ptrb200_ffnet* net, int x_dtype, int B, int n, int total_rows);
-int ptrb200_ffnet_forward_x(const ptrb200_ffnet* net, const void* X, int x_dtype, float* out, void* workspace,
-                            int64_t workspace_bytes, int B, int n, const int32_t* offsets, int total_rows, int training,
-                            uint64_t seed, uint64_t offset, ptrb200_stream_t stream);
-int ptrb200_ffnet_backward_x(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, const void* X, int x_dtype,
-                             const float* dOut, float* dX, void* workspace, int64_t workspace_bytes,
-                             int B, int n, const int32_t* offsets, int total_rows, int training, uint64_t seed, uint64_t offset,
-                             ptrb200_stream_t stream);
 
 /* ---- optimizer step ---------------------------------------------------------------------- */
 /* torch.optim.Adam.step() (ranker.py:512-525 -> config_optimizer; defaults betas=(0.9,0.999), eps=1e-8) over flat fp32
@@ -462,10 +448,14 @@ int ptrb200_rmsprop_step(float* param, const float* grad, float* square_avg, int
                          ptrb200_stream_t stream);
 
 /* Ragged <-> padded layout change for the list scorer (no counterpart: the reference batches equal-length lists only,
- * data_utils.py:683-742): padded[b, r, :] = flat[offsets[b] + r, :] for r < len_b, else 0; unpad is the inverse gather.
- * offsets: int32[B+1] prefix offsets, n_max: padded list length, F: row width (1 for score vectors). */
-int ptrb200_pad_lists(const float* flat, const int32_t* offsets, float* padded, int B, int n_max, int F,
-                      ptrb200_stream_t stream);
+ * data_utils.py:683-742).  offsets: int32 prefix offsets of the ragged rows, n_max: padded list length.
+ * ptrb200_pad_lists: padded query b is query q = qidx[b] of the offsets (qidx: B int32 on the device, or NULL for
+ * queries 0..B-1): padded[b, r, 0:W] = src[(offsets[q] + r) * ld_src + 0:W] for r < min(len_q, n_max), else 0 -- a
+ * strided column block of the rows (ld_src >= W; ld_src = W for whole rows, W = 1 for score vectors) into the dense
+ * [B, n_max, W] layout of the encoder.
+ * ptrb200_unpad_lists, the inverse gather: flat[offsets[b] + r, 0:F] = padded[b, r, 0:F] for r < min(len_b, n_max). */
+int ptrb200_pad_lists(const float* src, long long ld_src, const int32_t* offsets, const int32_t* qidx, float* padded,
+                      int B, int n_max, int W, ptrb200_stream_t stream);
 int ptrb200_unpad_lists(const float* padded, const int32_t* offsets, float* flat, int B, int n_max, int F,
                         ptrb200_stream_t stream);
 
@@ -505,31 +495,23 @@ int ptrb200_rmsprop_step_peer(const ptrb200_peer_group* grp, float* param, float
 /* MultiheadAttention.forward, ptranking/base/list_ranker.py:226-248: for every (query b, head h)
  * O = dropout(softmax(Q K^T / sqrt(D))) V.  Q,K,V,O: [B,n,H*D] with head h in columns [h*D,(h+1)*D) (the reference's
  * view/permute, :222-224, :251).  Every contraction is a batched wgmma GEMM in 3xTF32 (split operands, fp32-grade
- * results); `passes` must be 3, any other value returns PTRB200_ERR_UNSUPPORTED.  The attention matrix P[B*H,n,n]
- * is materialised in HBM and kept for the backward pass.  Dropout keeps element ((b*H+h)*n + i)*n + j of P with the
- * stream of PTRB200_EW_DROPOUT over a flat [B*H,n,n] tensor.
- * scratch: ptrb200_attention_tc_workspace_floats(B,n,H,D,backward) floats. */
-int64_t ptrb200_attention_tc_workspace_floats(int B, int n, int H, int D, int backward);
-int ptrb200_attention_tc_fwd(const float* Q, const float* K, const float* V, float* O, float* P_out, float* scratch,
-                             int B, int n, int H, int D, float dropout_p, uint64_t seed, uint64_t offset, int passes,
-                             ptrb200_stream_t stream);
+ * results).  The attention matrix P[B*H,n,n] is materialised in HBM and kept for the backward pass.  Dropout keeps
+ * element ((b*H+h)*n + i)*n + j of P with the stream of PTRB200_EW_DROPOUT over a flat [B*H,n,n] tensor.
+ * Operands may be row-pitched: ld_qkv = floats between consecutive documents of Q, K and V (and of dQ, dK, dV), ld_o =
+ * the same for O and dO; 0 = packed (H*D).  With Q|K|V side by side in one [B,n,3*H*D] tensor -- the output of ONE
+ * 136->408 projection instead of the reference's three (list_ranker.py:233-235) -- the call takes Q = qkv,
+ * K = qkv + H*D, V = qkv + 2*H*D, ld_qkv = 3*H*D, and the backward call fills the matching gradient tensor.
+ * key_lens (forward; NULL = every list has n documents): int32[B], query b attends to its first key_lens[b] documents only
+ * -- a ragged batch padded to n (ptrb200_pad_lists); masked probabilities are exactly 0, so the backward call needs nothing.
+ * scratch (backward): ptrb200_attention_tc_workspace_floats(B,n,H) floats. */
+int64_t ptrb200_attention_tc_workspace_floats(int B, int n, int H);
+int ptrb200_attention_tc_fwd(const float* Q, const float* K, const float* V, float* O, float* P_out,
+                             int B, int n, int H, int D, int ld_qkv, int ld_o, const int32_t* key_lens, float dropout_p,
+                             uint64_t seed, uint64_t offset, ptrb200_stream_t stream);
 int ptrb200_attention_tc_bwd(const float* Q, const float* K, const float* V, const float* P, const float* dO,
                              float* dQ, float* dK, float* dV, float* scratch,
-                             int B, int n, int H, int D, float dropout_p, uint64_t seed, uint64_t offset, int passes,
-                             ptrb200_stream_t stream);
-/* The same two calls over row-pitched operands: ld_qkv = floats between consecutive documents of Q, K and V (and of dQ,
- * dK, dV), ld_o = the same for O and dO; 0 = packed (H*D).  With Q|K|V side by side in one [B,n,3*H*D] tensor -- the
- * output of ONE 136->408 projection instead of the reference's three (list_ranker.py:233-235) -- the call takes
- * Q = qkv, K = qkv + H*D, V = qkv + 2*H*D, ld_qkv = 3*H*D, and the backward call fills the matching gradient tensor.
- * key_lens (forward; NULL = every list has n documents): int32[B], query b attends to its first key_lens[b] documents only
- * -- a ragged batch padded to n (ptrb200_pad_lists); masked probabilities are exactly 0, so the backward call needs nothing. */
-int ptrb200_attention_tc_fwd_ld(const float* Q, const float* K, const float* V, float* O, float* P_out, float* scratch,
-                                int B, int n, int H, int D, int ld_qkv, int ld_o, const int32_t* key_lens, float dropout_p,
-                                uint64_t seed, uint64_t offset, int passes, ptrb200_stream_t stream);
-int ptrb200_attention_tc_bwd_ld(const float* Q, const float* K, const float* V, const float* P, const float* dO,
-                                float* dQ, float* dK, float* dV, float* scratch,
-                                int B, int n, int H, int D, int ld_qkv, int ld_o, float dropout_p, uint64_t seed,
-                                uint64_t offset, int passes, ptrb200_stream_t stream);
+                             int B, int n, int H, int D, int ld_qkv, int ld_o, float dropout_p, uint64_t seed,
+                             uint64_t offset, ptrb200_stream_t stream);
 /* LayerNorm.forward, ptranking/base/list_ranker.py:165-174: y = a_2 (x - mean) / (std_unbiased + eps) + b_2 per row;
  * mean/std[rows] are kept for backward. */
 int ptrb200_layernorm_fwd(const float* x, const float* a2, const float* b2, float* y, float* mean, float* stdv,
@@ -556,16 +538,11 @@ int ptrb200_layernorm_bwd(const float* x, const float* a2, const float* dy, cons
 int ptrb200_elementwise(int op, const float* a, const float* b, float* out, int64_t count,
                         float dropout_p, uint64_t seed, uint64_t offset, ptrb200_stream_t stream);
 
-/* ---- tensor-core GEMM building block ---------------------------------------------------- */
-/* C[M,N] = A[M,K] * B[N,K]^T in fp32 through tf32 wgmma with register accumulation
- * (the contraction of nn.Linear: torch.nn.functional.linear as called by every ff_* layer of
- * get_stacked_FFNet, ptranking/base/utils.py:302,320).  passes = 1: plain TF32 operands;
- * passes = 3: error-compensated 3xTF32 (fp32-equivalent accuracy).  N <= 256. */
-int ptrb200_tc_gemm_nt(const float* A, const float* B, float* C, int M, int N, int K, int passes,
-                       ptrb200_stream_t stream);
-
-/* dW[N,K] = dZ[rows,N]^T * P[rows,K] (the weight gradient autograd forms for nn.Linear) with both operands
- * transposed into K-major wgmma operands; partials: 296*N*K floats of scratch.  N <= 128, K <= 256, K % 4 == 0. */
+/* ---- the scorer's tensor-core weight gradient on its own ---------------------------------------------------- */
+/* dW[N,K] = dZ[rows,N]^T * P[rows,K] (the weight gradient autograd forms for nn.Linear, get_stacked_FFNet,
+ * ptranking/base/utils.py:302,320) with both operands transposed into K-major wgmma operands; passes = 1: plain TF32
+ * operands, passes = 3: error-compensated 3xTF32 (fp32-equivalent accuracy); partials: 296*N*K floats of scratch.
+ * N <= 128, K <= 256, K % 4 == 0. */
 int ptrb200_tc_wgrad(const float* dZ, const float* P, float* dW, float* partials, int rows, int N, int K, int passes,
                      ptrb200_stream_t stream);
 

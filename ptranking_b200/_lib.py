@@ -22,7 +22,7 @@ MATH_MODES = {"simt": 0, "3xtf32": 1, "tf32": 2, "bf16": 3}
 LAMBDALOSS_TYPES = {"NDCG_Loss1": 0, "NDCG_Loss2": 1, "NDCG_Loss2++": 2}
 WASS_COST_TYPES = {"p1": 0, "p2": 1, "eg": 2, "dg": 3, "ddg": 4}   # PTRB200_WASS_COST_*
 MDP_DISTRIBUTIONS = {"PL": 0, "STPL": 1}                            # PTRB200_MDP_*
-DTYPE_F32, DTYPE_BF16 = 0, 1                                       # PTRB200_DTYPE_*: feature element type of the _x entries
+DTYPE_F32, DTYPE_BF16 = 0, 1                                       # PTRB200_DTYPE_*
 
 _fp = C.c_void_p   # device pointers travel as integers
 
@@ -84,40 +84,31 @@ SIGNATURES = {
                                        _F, _fp]),
     "ptrb200_div_features": (_I, [_fp, _fp, _fp, _fp, _I, _I, _I, _fp]),
     "ptrb200_div_list_features": (_I, [_fp, _fp, _fp, _fp, _I, _I, _I, _fp]),
-    "ptrb200_pad_lists_pitched": (_I, [_fp, _I64, _fp, _fp, _fp, _I, _I, _I, _fp]),
+    "ptrb200_pad_lists": (_I, [_fp, _I64, _fp, _fp, _fp, _I, _I, _I, _fp]),
     "ptrb200_div_list_concat": (_I, [_fp, _fp, _fp, _fp, _fp, _I, _I, _I, _fp]),
     "ptrb200_div_rerank_select": (_I, [_fp, _fp, _I, _I, _I, _fp, _fp, _fp, C.POINTER(C.c_int32), _fp]),
     "ptrb200_div_rerank_gather": (_I, [_fp, _I, _fp, _fp, _fp, _I, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
     "ptrb200_div_ideal_order": (_I, [_fp, _fp, _fp, _fp, _I, _I, _fp, _fp]),
     "ptrb200_div_pack_split": (_I, [_fp, _I, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _I, _F, _U64, _fp, _fp, _fp, _fp]),
-    "ptrb200_standard_scale": (_I, [_fp, _fp, _fp, _I, _I, _I, _I, _F, _fp]),
+    "ptrb200_standard_scale": (_I, [_fp, _fp, _fp, _I, _I, _I, _I, _I, _F, _fp]),
     "ptrb200_sum_f32": (_I, [_fp, _fp, _I, _fp]),
     "ptrb200_ndcg_at_ks": (_I, [_fp, _fp, _fp, C.POINTER(C.c_int32), _I, _fp, _fp, _I, _I, _I, _fp]),
     "ptrb200_adhoc_metrics_at_ks": (_I, [_fp, _fp, _fp, C.POINTER(C.c_int32), _I, _fp, _I, _I, _I, _F, _fp]),
     "ptrb200_adam_step": (_I, [_fp, _fp, _fp, _fp, _I64, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, _I, _fp]),
     "ptrb200_adagrad_step": (_I, [_fp, _fp, _fp, _I64, C.c_double, C.c_double, C.c_double, C.c_double, _I, _fp]),
     "ptrb200_rmsprop_step": (_I, [_fp, _fp, _fp, _I64, C.c_double, C.c_double, C.c_double, C.c_double, _fp]),
-    "ptrb200_attention_tc_workspace_floats": (_I64, [_I, _I, _I, _I, _I]),
-    "ptrb200_attention_tc_fwd": (_I, [_fp] * 6 + [_I, _I, _I, _I, _F, _U64, _U64, _I, _fp]),
-    "ptrb200_attention_tc_bwd": (_I, [_fp] * 9 + [_I, _I, _I, _I, _F, _U64, _U64, _I, _fp]),
-    "ptrb200_attention_tc_fwd_ld": (_I, [_fp] * 6 + [_I, _I, _I, _I, _I, _I, _fp, _F, _U64, _U64, _I, _fp]),
-    "ptrb200_pad_lists": (_I, [_fp, _fp, _fp, _I, _I, _I, _fp]),
+    "ptrb200_attention_tc_workspace_floats": (_I64, [_I, _I, _I]),
+    "ptrb200_attention_tc_fwd": (_I, [_fp] * 5 + [_I, _I, _I, _I, _I, _I, _fp, _F, _U64, _U64, _fp]),
+    "ptrb200_attention_tc_bwd": (_I, [_fp] * 9 + [_I, _I, _I, _I, _I, _I, _F, _U64, _U64, _fp]),
     "ptrb200_unpad_lists": (_I, [_fp, _fp, _fp, _I, _I, _I, _fp]),
-    "ptrb200_attention_tc_bwd_ld": (_I, [_fp] * 9 + [_I, _I, _I, _I, _I, _I, _F, _U64, _U64, _I, _fp]),
     "ptrb200_layernorm_fwd": (_I, [_fp, _fp, _fp, _fp, _fp, _fp, _I, _I, _F, _fp]),
     "ptrb200_layernorm_bwd": (_I, [_fp] * 9 + [_I, _I, _F, _fp]),
     "ptrb200_elementwise": (_I, [_I, _fp, _fp, _fp, _I64, _F, _U64, _U64, _fp]),
-    "ptrb200_tc_gemm_nt": (_I, [_fp, _fp, _fp, _I, _I, _I, _I, _fp]),
     "ptrb200_tc_wgrad": (_I, [_fp, _fp, _fp, _fp, _I, _I, _I, _I, _fp]),
-    "ptrb200_ffnet_workspace_bytes": (_I64, [C.POINTER(FFNetDesc), _I, _I, _I]),
-    "ptrb200_ffnet_forward": (_I, [C.POINTER(FFNetDesc), _fp, _fp, _fp, _I64, _I, _I, _fp, _I, _I, _U64, _U64, _fp]),
-    "ptrb200_ffnet_backward": (_I, [C.POINTER(FFNetDesc), C.POINTER(FFNetGrads), _fp, _fp, _fp, _fp, _I64,
+    "ptrb200_ffnet_workspace_bytes": (_I64, [C.POINTER(FFNetDesc), _I, _I, _I, _I]),
+    "ptrb200_ffnet_forward": (_I, [C.POINTER(FFNetDesc), _fp, _I, _fp, _fp, _I64, _I, _I, _fp, _I, _I, _U64, _U64, _fp]),
+    "ptrb200_ffnet_backward": (_I, [C.POINTER(FFNetDesc), C.POINTER(FFNetGrads), _fp, _I, _fp, _fp, _fp, _I64,
                                     _I, _I, _fp, _I, _I, _U64, _U64, _fp]),
-    "ptrb200_standard_scale_bf16": (_I, [_fp, _fp, _fp, _I, _I, _I, _I, _F, _fp]),
-    "ptrb200_ffnet_workspace_bytes_x": (_I64, [C.POINTER(FFNetDesc), _I, _I, _I, _I]),
-    "ptrb200_ffnet_forward_x": (_I, [C.POINTER(FFNetDesc), _fp, _I, _fp, _fp, _I64, _I, _I, _fp, _I, _I, _U64, _U64, _fp]),
-    "ptrb200_ffnet_backward_x": (_I, [C.POINTER(FFNetDesc), C.POINTER(FFNetGrads), _fp, _I, _fp, _fp, _fp, _I64,
-                                      _I, _I, _fp, _I, _I, _U64, _U64, _fp]),
 }
 
 

@@ -12,8 +12,8 @@
 // Two kernels implement the batched GEMM: bgemm_nt_tc_kernel takes any shape; bgemm_fast_kernel (every extent, pitch and
 // base address a multiple of four floats -- the attention core's own shapes) has the operand layouts and the dropout view
 // as template parameters, loads one K-chunk ahead and writes full-width tiles through shared memory; both produce the
-// same bits.  The row-pitched entry points (_ld) read Q|K|V side by side from one projection output and take per-query key
-// counts for padded ragged batches.
+// same bits.  The entry points take row pitches, so they read Q|K|V side by side from one projection output, and per-query
+// key counts for padded ragged batches.
 #include "common.cuh"
 #include "tc.cuh"
 
@@ -404,19 +404,14 @@ using namespace ptrb200;
 
 extern "C" {
 
-// scratch (floats): the backward pass needs dS[Z,n,n]; the forward pass none (a 4-float minimum keeps allocations non-empty)
-int64_t ptrb200_attention_tc_workspace_floats(int B, int n, int H, int D, int backward) {
-    const int64_t Z = (int64_t)B * H, nn = (int64_t)n * n;
-    (void)D;
-    return backward ? Z * nn : 4;
-}
+// the backward pass's scratch: dS[Z,n,n]
+int64_t ptrb200_attention_tc_workspace_floats(int B, int n, int H) { return (int64_t)B * H * n * n; }
 
 // P_out[B*H, n, n] receives the (un-dropped) attention probabilities and must be kept for the backward pass.
-int ptrb200_attention_tc_fwd_ld(const float* Q, const float* K, const float* V, float* O, float* P_out, float* scratch,
-                                int B, int n, int H, int D, int ld_qkv, int ld_o, const int32_t* key_lens, float dropout_p,
-                                uint64_t seed, uint64_t offset, int passes, ptrb200_stream_t stream) {
-    if (!Q || !K || !V || !O || !P_out || !scratch || B <= 0 || n <= 0 || H <= 0 || D <= 0) { set_error("attention_tc_fwd: bad arguments"); return PTRB200_ERR_INVALID; }
-    if (passes != 3) { set_error("attention_tc_fwd: passes must be 3 (3xTF32), got %d", passes); return PTRB200_ERR_UNSUPPORTED; }
+int ptrb200_attention_tc_fwd(const float* Q, const float* K, const float* V, float* O, float* P_out,
+                             int B, int n, int H, int D, int ld_qkv, int ld_o, const int32_t* key_lens, float dropout_p,
+                             uint64_t seed, uint64_t offset, ptrb200_stream_t stream) {
+    if (!Q || !K || !V || !O || !P_out || B <= 0 || n <= 0 || H <= 0 || D <= 0) { set_error("attention_tc_fwd: bad arguments"); return PTRB200_ERR_INVALID; }
     cudaStream_t st = (cudaStream_t)stream;
     const int Z = B * H, HD = H * D;
     const int lq = ld_qkv > 0 ? ld_qkv : HD, lo = ld_o > 0 ? ld_o : HD;
@@ -431,7 +426,6 @@ int ptrb200_attention_tc_fwd_ld(const float* Q, const float* K, const float* V, 
     const size_t rows = (size_t)Z * n;
     PTRB200_LAUNCH(softmax_rows_kernel, (unsigned)((rows + 7) / 8), 256, 0, st, P_out, rows, n, key_lens, H * n);
     // O = dropout(P) V : V is the [K = key, N = d] row-major factor, consumed MN-major
-    (void)scratch;
     BGemmArgs o{};
     o.A = P_out; o.B = V; o.C = O; o.M = n; o.N = D; o.K = n; o.lda = n; o.ldb = lq; o.ldc = lo; o.b_mn = 1;
     o.sAb = nn * H; o.sAh = nn; o.sBb = sb; o.sBh = sh; o.sCb = sbo; o.sCh = sh; o.H = H; o.alpha = 1.0f;
@@ -440,18 +434,11 @@ int ptrb200_attention_tc_fwd_ld(const float* Q, const float* K, const float* V, 
     return check_launch("attention_tc_fwd");
 }
 
-int ptrb200_attention_tc_fwd(const float* Q, const float* K, const float* V, float* O, float* P_out, float* scratch,
-                             int B, int n, int H, int D, float dropout_p, uint64_t seed, uint64_t offset, int passes,
-                             ptrb200_stream_t stream) {
-    return ptrb200_attention_tc_fwd_ld(Q, K, V, O, P_out, scratch, B, n, H, D, 0, 0, nullptr, dropout_p, seed, offset, passes, stream);
-}
-
-int ptrb200_attention_tc_bwd_ld(const float* Q, const float* K, const float* V, const float* P, const float* dO,
-                                float* dQ, float* dK, float* dV, float* scratch,
-                                int B, int n, int H, int D, int ld_qkv, int ld_o, float dropout_p, uint64_t seed,
-                                uint64_t offset, int passes, ptrb200_stream_t stream) {
+int ptrb200_attention_tc_bwd(const float* Q, const float* K, const float* V, const float* P, const float* dO,
+                             float* dQ, float* dK, float* dV, float* scratch,
+                             int B, int n, int H, int D, int ld_qkv, int ld_o, float dropout_p, uint64_t seed,
+                             uint64_t offset, ptrb200_stream_t stream) {
     if (!Q || !K || !V || !P || !dO || !dQ || !dK || !dV || !scratch || B <= 0 || n <= 0 || H <= 0 || D <= 0) { set_error("attention_tc_bwd: bad arguments"); return PTRB200_ERR_INVALID; }
-    if (passes != 3) { set_error("attention_tc_bwd: passes must be 3 (3xTF32), got %d", passes); return PTRB200_ERR_UNSUPPORTED; }
     cudaStream_t st = (cudaStream_t)stream;
     const int Z = B * H, HD = H * D;
     const int lq = ld_qkv > 0 ? ld_qkv : HD, lo = ld_o > 0 ? ld_o : HD;
@@ -485,13 +472,6 @@ int ptrb200_attention_tc_bwd_ld(const float* Q, const float* K, const float* V, 
     v.drop_mode = 2; v.drop = drop;
     if ((rc = launch_bgemm(v, Z, st, "attn_tc_dv"))) return rc;
     return check_launch("attention_tc_bwd");
-}
-
-int ptrb200_attention_tc_bwd(const float* Q, const float* K, const float* V, const float* P, const float* dO,
-                             float* dQ, float* dK, float* dV, float* scratch,
-                             int B, int n, int H, int D, float dropout_p, uint64_t seed, uint64_t offset, int passes,
-                             ptrb200_stream_t stream) {
-    return ptrb200_attention_tc_bwd_ld(Q, K, V, P, dO, dQ, dK, dV, scratch, B, n, H, D, 0, 0, dropout_p, seed, offset, passes, stream);
 }
 
 }  // extern "C"

@@ -83,7 +83,7 @@ int ptrb200_timing_report(char* buf, int buflen) {
     return PTRB200_OK;
 }
 
-int ptrb200_version(void) { return 100; }
+int ptrb200_version(void) { return 101; }
 
 const char* ptrb200_last_error(void) { return ptrb200::g_err; }
 

@@ -226,30 +226,21 @@ __global__ void div_list_features_kernel(const float* __restrict__ q_repr, const
     }
 }
 
-// A length class of a ragged batch: query b of the class is query qidx[b] (b when qidx is NULL) of the prefix offsets,
-// padded to n_max rows.  One CTA per (class query, row block), as pad_lists_kernel.
-//   PAD:  padded[b, r, 0:W] = src[(offsets[q] + r) * ld_src + 0:W] for r < len_q, 0 for len_q <= r < n_max
-//   !PAD: the scorer input of the class's rows: out[row, 0:W] = feats[row, 0:W], out[row, W:2W] = enc[b, r, 0:W]
-template <bool PAD>
-__global__ void div_list_rows_kernel(const float* __restrict__ src, long long ld_src, const float* __restrict__ enc,
-                                     const int32_t* __restrict__ offsets, const int32_t* __restrict__ qidx,
-                                     float* __restrict__ dst, int n_max, int W) {
+// The uni_sf input of a length class of a ragged batch: query b of the class is query qidx[b] (b when qidx is NULL) of the
+// prefix offsets, padded to n_max rows in enc.  One CTA per (class query, row block), as pad_lists_kernel.
+//   out[row, 0:W] = feats[row, 0:W], out[row, W:2W] = enc[b, r, 0:W]
+__global__ void div_list_concat_kernel(const float* __restrict__ feats, const float* __restrict__ enc,
+                                       const int32_t* __restrict__ offsets, const int32_t* __restrict__ qidx,
+                                       float* __restrict__ out, int n_max, int W) {
     const int b = blockIdx.x;
     const int q = qidx ? qidx[b] : b;
     const int base = offsets[q], n = min(offsets[q + 1] - base, n_max);
-    for (int r = blockIdx.y; r < (PAD ? n_max : n); r += gridDim.y) {
-        if (PAD) {
-            const float* s = src + (size_t)(base + r) * ld_src;
-            float* d = dst + ((size_t)b * n_max + r) * W;
-            const bool live = r < n;
-            for (int f = threadIdx.x; f < W; f += blockDim.x) d[f] = live ? s[f] : 0.0f;
-        } else {
-            const size_t row = (size_t)(base + r);
-            const float* s = src + row * W;
-            const float* e = enc + ((size_t)b * n_max + r) * W;
-            float* d = dst + row * 2 * W;
-            for (int f = threadIdx.x; f < W; f += blockDim.x) { d[f] = s[f]; d[W + f] = e[f]; }
-        }
+    for (int r = blockIdx.y; r < n; r += gridDim.y) {
+        const size_t row = (size_t)(base + r);
+        const float* s = feats + row * W;
+        const float* e = enc + ((size_t)b * n_max + r) * W;
+        float* d = out + row * 2 * W;
+        for (int f = threadIdx.x; f < W; f += blockDim.x) { d[f] = s[f]; d[W + f] = e[f]; }
     }
 }
 
@@ -320,27 +311,15 @@ int ptrb200_div_list_features(const float* q_repr, const float* docs, const int3
     return check_launch("div_list_features");
 }
 
-static inline int div_list_threads(int W) { return W >= 128 ? 128 : ((W + 31) / 32) * 32; }
-
-int ptrb200_pad_lists_pitched(const float* src, long long ld_src, const int32_t* offsets, const int32_t* qidx,
-                              float* padded, int B, int n_max, int W, ptrb200_stream_t stream) {
-    if (!src || !offsets || !padded || B <= 0 || n_max <= 0 || W <= 0 || ld_src < W) {
-        set_error("pad_lists_pitched: bad arguments (B=%d n_max=%d W=%d ld_src=%lld)", B, n_max, W, ld_src);
-        return PTRB200_ERR_INVALID;
-    }
-    PTRB200_LAUNCH_TAG("pad_lists_pitched_kernel", div_list_rows_kernel<true>, dim3(B, n_max < 64 ? n_max : 64), div_list_threads(W), 0, stream, src,
-                   ld_src, nullptr, offsets, qidx, padded, n_max, W);
-    return check_launch("pad_lists_pitched");
-}
-
 int ptrb200_div_list_concat(const float* feats, const float* enc, const int32_t* offsets, const int32_t* qidx, float* out,
                             int B, int n_max, int W, ptrb200_stream_t stream) {
     if (!feats || !enc || !offsets || !out || B <= 0 || n_max <= 0 || W <= 0) {
         set_error("div_list_concat: bad arguments (B=%d n_max=%d W=%d)", B, n_max, W);
         return PTRB200_ERR_INVALID;
     }
-    PTRB200_LAUNCH_TAG("div_list_concat_kernel", div_list_rows_kernel<false>, dim3(B, n_max < 64 ? n_max : 64), div_list_threads(W), 0, stream, feats,
-                   (long long)W, enc, offsets, qidx, out, n_max, W);
+    const int threads = W >= 128 ? 128 : ((W + 31) / 32) * 32;
+    PTRB200_LAUNCH(div_list_concat_kernel, dim3(B, n_max < 64 ? n_max : 64), threads, 0, stream, feats, enc, offsets, qidx, out,
+                   n_max, W);
     return check_launch("div_list_concat");
 }
 

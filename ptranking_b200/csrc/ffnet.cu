@@ -1,5 +1,5 @@
 // ffnet.cu -- stacked feed-forward scorer: Dropout -> Linear -> (BN | BN2) -> activation, repeated,
-// forward and backward, fp32 SIMT path (the tensor-core kernels live in ffnet_tc.cuh and gemm_tc.cu).
+// forward and backward, fp32 SIMT path (the tensor-core kernels live in ffnet_tc.cuh).
 //
 // Reference functions replaced (wildltr/ptranking @ f1d366c):
 //   get_stacked_FFNet            ptranking/base/utils.py:288-356
@@ -1377,14 +1377,10 @@ int ptrb200_tc_wgrad(const float* dZ, const float* P, float* dW, float* partials
     return rc ? rc : check_launch("tc_wgrad");
 }
 
-int64_t ptrb200_ffnet_workspace_bytes_x(const ptrb200_ffnet* net, int x_dtype, int B, int n, int total_rows) {
+int64_t ptrb200_ffnet_workspace_bytes(const ptrb200_ffnet* net, int x_dtype, int B, int n, int total_rows) {
     Plan p;
     const int rc = make_plan(net, B, n, p, total_rows, x_dtype);
     return rc ? (int64_t)rc : (int64_t)p.total;
-}
-
-int64_t ptrb200_ffnet_workspace_bytes(const ptrb200_ffnet* net, int B, int n, int total_rows) {
-    return ptrb200_ffnet_workspace_bytes_x(net, PTRB200_DTYPE_F32, B, n, total_rows);
 }
 
 // a bf16 feature matrix is read 4 elements (8 bytes) at a time
@@ -1396,9 +1392,9 @@ static int check_x(const void* X, int x_dtype, const char* who) {
     return PTRB200_OK;
 }
 
-int ptrb200_ffnet_forward_x(const ptrb200_ffnet* net, const void* Xv, int x_dtype, float* out, void* workspace,
-                            int64_t workspace_bytes, int B, int n, const int32_t* offsets, int total_rows, int training,
-                            uint64_t seed, uint64_t offset, ptrb200_stream_t stream) {
+int ptrb200_ffnet_forward(const ptrb200_ffnet* net, const void* Xv, int x_dtype, float* out, void* workspace,
+                          int64_t workspace_bytes, int B, int n, const int32_t* offsets, int total_rows, int training,
+                          uint64_t seed, uint64_t offset, ptrb200_stream_t stream) {
     Plan p;
     if ((offsets != nullptr) != (total_rows > 0)) { set_error("ffnet_forward: offsets and total_rows go together (ragged batch) or are both absent"); return PTRB200_ERR_INVALID; }
     int rc = make_plan(net, B, n, p, total_rows, x_dtype);
@@ -1463,17 +1459,10 @@ int ptrb200_ffnet_forward_x(const ptrb200_ffnet* net, const void* Xv, int x_dtyp
     return check_launch("ffnet_forward");
 }
 
-int ptrb200_ffnet_forward(const ptrb200_ffnet* net, const float* X, float* out, void* workspace,
-                          int64_t workspace_bytes, int B, int n, const int32_t* offsets, int total_rows, int training,
-                          uint64_t seed, uint64_t offset, ptrb200_stream_t stream) {
-    return ptrb200_ffnet_forward_x(net, X, PTRB200_DTYPE_F32, out, workspace, workspace_bytes, B, n, offsets, total_rows, training,
-                                   seed, offset, stream);
-}
-
-int ptrb200_ffnet_backward_x(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, const void* Xv, int x_dtype,
-                             const float* dOut, float* dX, void* workspace, int64_t workspace_bytes,
-                             int B, int n, const int32_t* offsets, int total_rows, int training, uint64_t seed, uint64_t offset,
-                             ptrb200_stream_t stream) {
+int ptrb200_ffnet_backward(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, const void* Xv, int x_dtype,
+                           const float* dOut, float* dX, void* workspace, int64_t workspace_bytes,
+                           int B, int n, const int32_t* offsets, int total_rows, int training, uint64_t seed, uint64_t offset,
+                           ptrb200_stream_t stream) {
     Plan p;
     if ((offsets != nullptr) != (total_rows > 0)) { set_error("ffnet_backward: offsets and total_rows go together (ragged batch) or are both absent"); return PTRB200_ERR_INVALID; }
     int rc = make_plan(net, B, n, p, total_rows, x_dtype);
@@ -1571,14 +1560,6 @@ int ptrb200_ffnet_backward_x(const ptrb200_ffnet* net, const ptrb200_ffnet_grads
         }
     }
     return check_launch("ffnet_backward");
-}
-
-int ptrb200_ffnet_backward(const ptrb200_ffnet* net, const ptrb200_ffnet_grads* grads, const float* X,
-                           const float* dOut, float* dX, void* workspace, int64_t workspace_bytes,
-                           int B, int n, const int32_t* offsets, int total_rows, int training, uint64_t seed, uint64_t offset,
-                           ptrb200_stream_t stream) {
-    return ptrb200_ffnet_backward_x(net, grads, X, PTRB200_DTYPE_F32, dOut, dX, workspace, workspace_bytes, B, n, offsets,
-                                    total_rows, training, seed, offset, stream);
 }
 
 }  // extern "C"

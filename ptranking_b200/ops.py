@@ -437,12 +437,9 @@ def standard_scale(X: torch.Tensor, offsets: Optional[torch.Tensor] = None, max_
                                           or out.device != X.device):
         raise ValueError(f"out must be a contiguous {out_dtype} tensor of shape {tuple(X.shape)} on {X.device}")
     clip, cmax = int(clip_max is not None), float(clip_max if clip_max is not None else 0.0)
-    if out_dtype == torch.bfloat16:
-        _lib.check(lib.ptrb200_standard_scale_bf16(X.data_ptr(), op, out.data_ptr(), B, n, F, clip, cmax, _stream_ptr()),
-                   "standard_scale_bf16")
-    else:
-        _lib.check(lib.ptrb200_standard_scale(X.data_ptr(), op, out.data_ptr(), B, n, F, clip, cmax, _stream_ptr()),
-                   "standard_scale")
+    code = _lib.DTYPE_BF16 if out_dtype == torch.bfloat16 else _lib.DTYPE_F32
+    _lib.check(lib.ptrb200_standard_scale(X.data_ptr(), op, out.data_ptr(), code, B, n, F, clip, cmax, _stream_ptr()),
+               "standard_scale")
     return out
 
 
@@ -907,8 +904,8 @@ def pad_lists_pitched(src: torch.Tensor, offsets: torch.Tensor, qidx: torch.Tens
         raise ValueError(f"columns [{col0}, {col0 + width}) outside a row of {src.shape[1]}")
     op, qp = _class_ptrs(offsets, qidx, src.device)
     out = torch.empty((qidx.numel(), int(n_max), width), dtype=torch.float32, device=src.device)
-    _lib.check(lib.ptrb200_pad_lists_pitched(src.data_ptr() + 4 * col0, src.shape[1], op, qp, out.data_ptr(), qidx.numel(),
-                                             int(n_max), width, _stream_ptr()), "pad_lists_pitched")
+    _lib.check(lib.ptrb200_pad_lists(src.data_ptr() + 4 * col0, src.shape[1], op, qp, out.data_ptr(), qidx.numel(),
+                                     int(n_max), width, _stream_ptr()), "pad_lists")
     return out
 
 
@@ -1052,7 +1049,7 @@ class _FFNetFn(torch.autograd.Function):
             raise ValueError(f"feature width {F} != net input width {spec.dims[0]}")
         params = [p.detach().contiguous() for p in params]
         desc = spec.describe(params)
-        nbytes = lib.ptrb200_ffnet_workspace_bytes_x(C.byref(desc), x_dtype, B, n, total)
+        nbytes = lib.ptrb200_ffnet_workspace_bytes(C.byref(desc), x_dtype, B, n, total)
         if nbytes < 0:
             _lib.check(int(nbytes), "ffnet_workspace_bytes")
         ws = torch.empty(int(nbytes), dtype=torch.uint8, device=X.device)
@@ -1061,8 +1058,8 @@ class _FFNetFn(torch.autograd.Function):
         # caller runs under torch.no_grad()), so the by-products the backward pass reads are not written
         flags = int(training) | (0 if need_backward else 2)
         with _b200dist().call_context(ws, None):
-            _lib.check(lib.ptrb200_ffnet_forward_x(C.byref(desc), X.data_ptr(), x_dtype, out.data_ptr(), ws.data_ptr(),
-                                                   int(nbytes), B, n, op, total, flags, seed, offset, _stream_ptr()),
+            _lib.check(lib.ptrb200_ffnet_forward(C.byref(desc), X.data_ptr(), x_dtype, out.data_ptr(), ws.data_ptr(),
+                                                 int(nbytes), B, n, op, total, flags, seed, offset, _stream_ptr()),
                        "ffnet_forward")
         ctx.spec, ctx.training, ctx.seed, ctx.offset, ctx.x_dtype = spec, training, seed, offset, x_dtype
         ctx.shape = (B, n, offsets, total)
@@ -1093,10 +1090,10 @@ class _FFNetFn(torch.autograd.Function):
                 layer_targets.append(gouts[i: i + len(names)])
                 i += len(names)
         with _b200dist().call_context(ctx.ws, layer_targets):
-            _lib.check(lib.ptrb200_ffnet_backward_x(C.byref(desc), C.byref(gdesc), X.data_ptr(), ctx.x_dtype, d_out.data_ptr(),
-                                                    dX.data_ptr() if dX is not None else None, ctx.ws.data_ptr(), ctx.nbytes,
-                                                    B, n, offsets.data_ptr() if offsets is not None else None, total,
-                                                    int(ctx.training), ctx.seed, ctx.offset, _stream_ptr()),
+            _lib.check(lib.ptrb200_ffnet_backward(C.byref(desc), C.byref(gdesc), X.data_ptr(), ctx.x_dtype, d_out.data_ptr(),
+                                                  dX.data_ptr() if dX is not None else None, ctx.ws.data_ptr(), ctx.nbytes,
+                                                  B, n, offsets.data_ptr() if offsets is not None else None, total,
+                                                  int(ctx.training), ctx.seed, ctx.offset, _stream_ptr()),
                        "ffnet_backward")
         ctx.ws = None
         if ctx.grad_targets is not None:            # written straight into the parameters' .grad storage
@@ -1163,7 +1160,8 @@ class _PadLists(torch.autograd.Function):
         F = flat.shape[1] if flat.dim() == 2 else 1
         B = offsets.numel() - 1
         out = torch.empty((B, n_max, F) if flat.dim() == 2 else (B, n_max), dtype=torch.float32, device=flat.device)
-        _lib.check(lib.ptrb200_pad_lists(flat.data_ptr(), offsets.data_ptr(), out.data_ptr(), B, n_max, F, _stream_ptr()), "pad_lists")
+        _lib.check(lib.ptrb200_pad_lists(flat.data_ptr(), F, offsets.data_ptr(), None, out.data_ptr(), B, n_max, F, _stream_ptr()),
+                   "pad_lists")
         ctx.save_for_backward(offsets)
         ctx.shape = tuple(flat.shape)
         return out
@@ -1178,35 +1176,6 @@ class _PadLists(torch.autograd.Function):
         out = torch.zeros(ctx.shape, dtype=torch.float32, device=g.device)     # offsets may address a sub-range of the rows
         _lib.check(lib.ptrb200_unpad_lists(g.data_ptr(), offsets.data_ptr(), out.data_ptr(), offsets.numel() - 1, g.shape[1], F,
                                            _stream_ptr()), "unpad_lists")
-        return out, None, None
-
-
-class _UnpadLists(torch.autograd.Function):
-    """padded [B, n_max(, F)] -> flat [total(, F)]; backward pads the gradient (zeros at the padding)."""
-
-    @staticmethod
-    @_on_tensor_device
-    def forward(ctx, padded, offsets, total):
-        lib = _lib.load()
-        padded = _dev_f32(padded, "padded")
-        F = padded.shape[2] if padded.dim() == 3 else 1
-        B, n_max = padded.shape[0], padded.shape[1]
-        out = torch.empty((total, F) if padded.dim() == 3 else (total,), dtype=torch.float32, device=padded.device)
-        _lib.check(lib.ptrb200_unpad_lists(padded.data_ptr(), offsets.data_ptr(), out.data_ptr(), B, n_max, F, _stream_ptr()), "unpad_lists")
-        ctx.save_for_backward(offsets)
-        ctx.shape = tuple(padded.shape)
-        return out
-
-    @staticmethod
-    @_on_tensor_device
-    def backward(ctx, g):
-        (offsets,) = ctx.saved_tensors
-        lib = _lib.load()
-        g = _dev_f32(g, "g")
-        F = ctx.shape[2] if len(ctx.shape) == 3 else 1
-        out = torch.empty(ctx.shape, dtype=torch.float32, device=g.device)
-        _lib.check(lib.ptrb200_pad_lists(g.data_ptr(), offsets.data_ptr(), out.data_ptr(), ctx.shape[0], ctx.shape[1], F,
-                                         _stream_ptr()), "pad_lists")
         return out, None, None
 
 
@@ -1237,8 +1206,8 @@ class _UnpadBuckets(torch.autograd.Function):
         outs = []
         for q0, shp in zip(ctx.q0s, ctx.shapes):
             o = torch.empty(shp, dtype=torch.float32, device=g.device)
-            _lib.check(lib.ptrb200_pad_lists(g.data_ptr(), offsets.data_ptr() + 4 * q0, o.data_ptr(), shp[0], shp[1], ctx.F,
-                                             _stream_ptr()), "pad_lists")
+            _lib.check(lib.ptrb200_pad_lists(g.data_ptr(), ctx.F, offsets.data_ptr() + 4 * q0, None, o.data_ptr(), shp[0], shp[1],
+                                             ctx.F, _stream_ptr()), "pad_lists")
             outs.append(o)
         return (None, None, None, *outs)
 
@@ -1264,7 +1233,7 @@ def pad_lists(flat: torch.Tensor, offsets: torch.Tensor, n_max: int) -> torch.Te
 
 def unpad_lists(padded: torch.Tensor, offsets: torch.Tensor, total: int) -> torch.Tensor:
     """Inverse of :func:`pad_lists`: the first len_b rows of every list, concatenated (differentiable)."""
-    return _UnpadLists.apply(padded, _offsets_i32(offsets, padded.device), int(total))
+    return unpad_buckets([padded], offsets, total, [0])
 
 
 def _key_lens_ptr(B: int, device):
@@ -1318,11 +1287,10 @@ class _AttentionTCPacked(torch.autograd.Function):
         D = F // n_heads
         O = torch.empty((B, n, F), dtype=torch.float32, device=qkv.device)
         P = torch.empty((B * n_heads, n, n), dtype=torch.float32, device=qkv.device)
-        scratch = torch.empty(lib.ptrb200_attention_tc_workspace_floats(B, n, n_heads, D, 0), dtype=torch.float32, device=qkv.device)
         q = qkv.data_ptr()
-        _lib.check(lib.ptrb200_attention_tc_fwd_ld(q, q + 4 * F, q + 8 * F, O.data_ptr(), P.data_ptr(), scratch.data_ptr(),
-                                                   B, n, n_heads, D, F3, 0, _key_lens_ptr(B, qkv.device), float(dropout_p), seed, offset,
-                                                   3, _stream_ptr()), "attention_tc_fwd")
+        _lib.check(lib.ptrb200_attention_tc_fwd(q, q + 4 * F, q + 8 * F, O.data_ptr(), P.data_ptr(),
+                                                B, n, n_heads, D, F3, 0, _key_lens_ptr(B, qkv.device), float(dropout_p), seed, offset,
+                                                _stream_ptr()), "attention_tc_fwd")
         ctx.save_for_backward(qkv, P)
         ctx.cfg = (n_heads, float(dropout_p), seed, offset)
         return O
@@ -1337,11 +1305,11 @@ class _AttentionTCPacked(torch.autograd.Function):
         F = F3 // 3
         dO = _dev_f32(dO, "dO")
         dqkv = torch.empty_like(qkv)
-        scratch = torch.empty(lib.ptrb200_attention_tc_workspace_floats(B, n, H, F // H, 1), dtype=torch.float32, device=qkv.device)
+        scratch = torch.empty(lib.ptrb200_attention_tc_workspace_floats(B, n, H), dtype=torch.float32, device=qkv.device)
         q, g = qkv.data_ptr(), dqkv.data_ptr()
-        _lib.check(lib.ptrb200_attention_tc_bwd_ld(q, q + 4 * F, q + 8 * F, P.data_ptr(), dO.data_ptr(),
-                                                   g, g + 4 * F, g + 8 * F, scratch.data_ptr(),
-                                                   B, n, H, F // H, F3, 0, p, seed, offset, 3, _stream_ptr()), "attention_tc_bwd")
+        _lib.check(lib.ptrb200_attention_tc_bwd(q, q + 4 * F, q + 8 * F, P.data_ptr(), dO.data_ptr(),
+                                                g, g + 4 * F, g + 8 * F, scratch.data_ptr(),
+                                                B, n, H, F // H, F3, 0, p, seed, offset, _stream_ptr()), "attention_tc_bwd")
         return dqkv, None, None, None, None
 
 

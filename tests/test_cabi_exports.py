@@ -37,27 +37,20 @@ def test_ctypes_prototypes_match_header(lib_path):
     from ptranking_b200 import _lib
     assert sorted(_lib.SIGNATURES) == header_symbols()
     lib = _lib.load()
-    assert lib.ptrb200_version() >= 100
+    assert lib.ptrb200_version() >= 101
     assert isinstance(lib.ptrb200_launch_count(), int)
 
 
-def test_attention_tc_entry_points_reject_passes_other_than_3(lib_path):
-    """The attention calls keep their `passes` argument for ABI stability; only 3 (3xTF32) is implemented, and any other
-    value is refused while the arguments are checked, before anything reaches the device."""
+def test_standard_scale_refuses_unknown_dtype_and_aliased_bf16_output(lib_path):
+    """The output element type is checked with the arguments, before anything reaches the device."""
     from ptranking_b200 import _lib
     lib = _lib.load()
     buf = (ctypes.c_float * 16)()
     p = ctypes.addressof(buf)          # never dereferenced: the call returns at the argument check
-    B, n, H, D = 1, 4, 1, 4
-    calls = {
-        "attention_tc_fwd": lambda: lib.ptrb200_attention_tc_fwd(*[p] * 6, B, n, H, D, 0.0, 0, 0, 1, None),
-        "attention_tc_bwd": lambda: lib.ptrb200_attention_tc_bwd(*[p] * 9, B, n, H, D, 0.0, 0, 0, 1, None),
-        "attention_tc_fwd_ld": lambda: lib.ptrb200_attention_tc_fwd_ld(*[p] * 6, B, n, H, D, 0, 0, None, 0.0, 0, 0, 1, None),
-        "attention_tc_bwd_ld": lambda: lib.ptrb200_attention_tc_bwd_ld(*[p] * 9, B, n, H, D, 0, 0, 0.0, 0, 0, 1, None),
-    }
-    for name, call in calls.items():
-        with pytest.raises(_lib.B200LibraryError, match="passes must be 3"):
-            _lib.check(call(), name)
+    assert lib.ptrb200_standard_scale(p, None, p, 7, 1, 4, 4, 0, 0.0, None) == -1
+    assert b"out_dtype" in lib.ptrb200_last_error()
+    assert lib.ptrb200_standard_scale(p, None, p, _lib.DTYPE_BF16, 1, 4, 4, 0, 0.0, None) == -1
+    assert b"alias" in lib.ptrb200_last_error()
 
 
 def test_no_cpu_fallback():

@@ -182,7 +182,7 @@ def _ffnet_desc(spec, params):
     return spec.describe([q.detach().contiguous() for q in params])
 
 
-def test_bf16_abi_refuses_misaligned_and_unknown_dtype():
+def test_ffnet_entry_points_refuse_misaligned_bf16_and_unknown_dtype():
     from ptranking_b200 import _lib, ops
     lib = _lib.load()
     dims = [136, 100, 1]
@@ -192,24 +192,24 @@ def test_bf16_abi_refuses_misaligned_and_unknown_dtype():
     B, n = 2, 64
     Xb = torch.randn(B * n * 136 + 4, device=DEV).to(torch.bfloat16)
     out = torch.empty(B, n, 1, device=DEV)
-    nbytes = lib.ptrb200_ffnet_workspace_bytes_x(C.byref(desc), _lib.DTYPE_BF16, B, n, 0)
+    nbytes = lib.ptrb200_ffnet_workspace_bytes(C.byref(desc), _lib.DTYPE_BF16, B, n, 0)
     assert nbytes > 0
     ws = torch.empty(int(nbytes), dtype=torch.uint8, device=DEV)
     stream = torch.cuda.current_stream().cuda_stream
-    ok = lib.ptrb200_ffnet_forward_x(C.byref(desc), Xb.data_ptr(), _lib.DTYPE_BF16, out.data_ptr(), ws.data_ptr(), int(nbytes),
-                                     B, n, None, 0, 0, 1, 1, stream)
+    ok = lib.ptrb200_ffnet_forward(C.byref(desc), Xb.data_ptr(), _lib.DTYPE_BF16, out.data_ptr(), ws.data_ptr(), int(nbytes),
+                                   B, n, None, 0, 0, 1, 1, stream)
     assert ok == 0
-    rc = lib.ptrb200_ffnet_forward_x(C.byref(desc), Xb.data_ptr() + 2, _lib.DTYPE_BF16, out.data_ptr(), ws.data_ptr(), int(nbytes),
-                                     B, n, None, 0, 0, 1, 1, stream)
+    rc = lib.ptrb200_ffnet_forward(C.byref(desc), Xb.data_ptr() + 2, _lib.DTYPE_BF16, out.data_ptr(), ws.data_ptr(), int(nbytes),
+                                   B, n, None, 0, 0, 1, 1, stream)
     assert rc == -1 and b"aligned" in lib.ptrb200_last_error()
-    rc = lib.ptrb200_ffnet_forward_x(C.byref(desc), Xb.data_ptr(), 7, out.data_ptr(), ws.data_ptr(), int(nbytes),
-                                     B, n, None, 0, 0, 1, 1, stream)
+    rc = lib.ptrb200_ffnet_forward(C.byref(desc), Xb.data_ptr(), 7, out.data_ptr(), ws.data_ptr(), int(nbytes),
+                                   B, n, None, 0, 0, 1, 1, stream)
     assert rc == -1 and b"dtype" in lib.ptrb200_last_error()
-    assert lib.ptrb200_ffnet_workspace_bytes_x(C.byref(desc), 7, B, n, 0) == -1
+    assert lib.ptrb200_ffnet_workspace_bytes(C.byref(desc), 7, B, n, 0) == -1
     gdesc, _ = spec.grads([q.detach() for q in params])
     dO = torch.randn(B, n, 1, device=DEV)
-    rc = lib.ptrb200_ffnet_backward_x(C.byref(desc), C.byref(gdesc), Xb.data_ptr() + 2, _lib.DTYPE_BF16, dO.data_ptr(), None,
-                                      ws.data_ptr(), int(nbytes), B, n, None, 0, 0, 1, 1, stream)
+    rc = lib.ptrb200_ffnet_backward(C.byref(desc), C.byref(gdesc), Xb.data_ptr() + 2, _lib.DTYPE_BF16, dO.data_ptr(), None,
+                                    ws.data_ptr(), int(nbytes), B, n, None, 0, 0, 1, 1, stream)
     assert rc == -1 and b"aligned" in lib.ptrb200_last_error()
     torch.cuda.synchronize()
 

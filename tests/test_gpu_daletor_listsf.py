@@ -116,15 +116,15 @@ def test_pad_lists_pitched_and_concat_against_torch_indexing():
             assert (blk.grad[b, lens[q]:] == 0).all()                       # exact zeros at padding
 
 
-def test_new_entry_points_reject_bad_arguments():
+def test_list_scorer_row_entry_points_reject_bad_arguments():
     from ptranking_b200 import _lib
     lib = _lib.load()
     x = torch.zeros(8, device=DEV)
     p = x.data_ptr()
     assert lib.ptrb200_div_list_features(p, p, None, p, 0, 4, 2, None) != 0             # B = 0
     assert lib.ptrb200_div_list_features(None, p, None, p, 1, 4, 2, None) != 0
-    assert lib.ptrb200_pad_lists_pitched(p, 1, p, None, p, 1, 4, 2, None) != 0          # ld_src < W
-    assert lib.ptrb200_pad_lists_pitched(p, 2, None, None, p, 1, 4, 2, None) != 0       # no offsets
+    assert lib.ptrb200_pad_lists(p, 1, p, None, p, 1, 4, 2, None) != 0                  # ld_src < W
+    assert lib.ptrb200_pad_lists(p, 2, None, None, p, 1, 4, 2, None) != 0               # no offsets
     assert lib.ptrb200_div_list_concat(p, None, p, None, p, 1, 4, 2, None) != 0         # no encoder block
     assert lib.ptrb200_div_list_concat(p, p, p, None, p, 1, 0, 2, None) != 0            # n_max = 0
     assert b"div_list_concat" in lib.ptrb200_last_error()

@@ -378,3 +378,21 @@ def test_list_scorer_ragged_batch_equals_query_by_query(enc):
     P = ops.pad_lists(X, offd, max(lens))
     assert P.shape == (len(lens), max(lens), F) and torch.equal(ops.unpad_lists(P, offd, sum(lens)), X)
     assert float(P[1, lens[1]:].abs().max()) == 0.0
+
+
+def test_unpad_lists_stops_at_the_padded_block():
+    """A list longer than the padded length gives back only the n_max rows its block holds; its rows behind stay
+    untouched."""
+    from ptranking_b200 import _lib
+    lib = _lib.load()
+    lens, n_max, F = [9, 3, 5], 5, 4
+    o = np.concatenate([[0], np.cumsum(lens)])
+    offd = torch.tensor(o, dtype=torch.int32, device=DEV)
+    padded = torch.arange(len(lens) * n_max * F, dtype=torch.float32, device=DEV).reshape(len(lens), n_max, F)
+    flat = torch.full((sum(lens), F), -1.0, device=DEV)
+    _lib.check(lib.ptrb200_unpad_lists(padded.data_ptr(), offd.data_ptr(), flat.data_ptr(), len(lens), n_max, F,
+                                       torch.cuda.current_stream().cuda_stream), "unpad_lists")
+    want = torch.full_like(flat, -1.0)
+    for b, n in enumerate(lens):
+        want[o[b]:o[b] + min(n, n_max)] = padded[b, :min(n, n_max)]
+    assert torch.equal(flat, want)

@@ -1,6 +1,7 @@
-"""The weight-gradient kernel (wgrad_tc) keeps one row tile's MMAs in flight while it stages the next tile into the
-other operand buffer.  A race on the operand buffers shows up as wrong or run-to-run different gradients, so every case
-is compared against float64 and run twice for bit equality, at row counts that give the persistent CTAs 0, 1, 2, ...
+"""The weight-gradient kernel (wgrad_tc) against float64, called on its own (ptrb200_tc_wgrad) and inside the scorer.
+It keeps one row tile's MMAs in flight while it stages the next tile into the other operand buffer.  A race on the
+operand buffers shows up as wrong or run-to-run different gradients, so the pipeline cases are also run twice for bit
+equality, at row counts that give the persistent CTAs 0, 1, 2, ...
 tiles up to one more than the raw-ring depth, with a short last tile."""
 import numpy as np
 import pytest
@@ -36,6 +37,21 @@ def _tc_wgrad(dZ, P, passes):
     _lib.check(lib.ptrb200_tc_wgrad(dZ.data_ptr(), P.data_ptr(), out.data_ptr(), part.data_ptr(), rows, N, K, passes,
                                     torch.cuda.current_stream().cuda_stream), "tc_wgrad")
     return out
+
+
+@pytest.mark.parametrize("shape", [(32, 100, 136), (64, 8, 32), (1000, 100, 100), (4096, 1, 100), (37, 128, 256), (5000, 100, 136)])
+def test_tc_wgrad_matches_float64(shape):
+    """dW = dZ^T P through operands transposed into K-major wgmma tiles while they are staged."""
+    rows, N, K = shape
+    g = torch.Generator(device="cpu").manual_seed(rows + N + K)
+    dZ = torch.randn(rows, N, generator=g).to(DEV)
+    P = torch.randn(rows, K, generator=g).to(DEV)
+    ref = dZ.double().t() @ P.double()
+    for passes, tol in ((3, 5e-6), (1, 5e-3)):
+        out = _tc_wgrad(dZ, P, passes)
+        torch.cuda.synchronize()
+        err = float((out.double() - ref).abs().max()) / float(ref.abs().max())
+        assert err <= tol, (shape, passes, err)
 
 
 @pytest.mark.parametrize("N", [1, 100, 128])

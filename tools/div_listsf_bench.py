@@ -85,7 +85,7 @@ def time_eval(r, data, reps):
     return a.elapsed_time(b) / reps
 
 
-GROUPS = [("new list-scorer kernels", ("div_list", "pad_lists_pitched", "div_list_rows")),
+GROUPS = [("new list-scorer kernels", ("div_list", "pad_lists")),
           ("attention GEMMs", ("bgemm", "attn_gemm", "attention_tc", "attn_mma")),
           ("softmax", ("softmax",)),
           ("LayerNorm", ("layernorm",)),
